@@ -1,8 +1,8 @@
 #!/usr/bin/env python3
 """bench.py -- headline benchmark of the create_proof hot path (BASELINE.json configs[1]):
-BN254 G1 Pippenger MSM over 2^20 random points / uniform scalars per GPU, B200 vs the CPU best_multiexp.
+BN254 G1 Pippenger MSM over 2^20 random points / uniform scalars per GPU (H100), vs the CPU best_multiexp.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P bench.py --gpus N ...
 
 One "step" = one batch of MSMS_PER_STEP = 16 commitments, each an MSM of n = 2^20 pairs per GPU against a resident basis
@@ -16,14 +16,19 @@ Every N prints `parity` flags: the folded result of a timed step is compared wit
 known discrete logs of the bases (sum_i s_i * h_i) * G1; the sharded 2^23 MSM with the single-GPU one; the multi-device
 NTT and proof with their single-device outputs, bit for bit.
 
-Extra keys: `roofline` (dominant kernel msm_accumulate_kernel vs measured HBM peak, plus the INT32-pipe view that
-actually binds it, plus the HBM-class quotient kernels), `cpu_baseline` (the oracle port of halo2's best_multiexp on this
+Extra keys: `roofline` (dominant kernel msm_accumulate_kernel vs the HBM peak, plus the INT32-pipe view that actually
+binds it, plus the HBM-class quotient kernels), `cpu_baseline` (the oracle port of halo2's best_multiexp on this
 box's cores, median of 5 after a full-size warm-up), `msm_sizes` (2^20 / 2^23 / 2^24 x scalar distributions),
 `strong_scaling` (one 2^23 MSM on 1 GPU vs sharded over N), `ntt` (2^20 / 2^22 / 2^23 / 2^25; six-step across N devices),
 `proof` (create_proof wall time: Python driver, compiled driver, N-device context), `stages_ms`, `clocks`, `gpu_launches`.
 
 --impl reference times the CPU restatement of the reference's own path (oracle/_ref; the Rust crates cannot be
-built in this image -- DESIGN.md) on the same workload.
+built without a cargo host -- DESIGN.md) on the same workload.
+
+--dump-outputs DIR writes, after the timed steps, the 16 commitments of the last timed step (the points a caller of
+spb_msm_batch_dev receives, folded over the ranks) as DIR/msm_commitments_affine.npy: float64, shape (16, 2, 8) = affine
+(x, y) as eight little-endian 32-bit limbs of the canonical integer each. Inputs are seeded, so two builds given the
+same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -42,7 +47,7 @@ sys.path.insert(0, ROOT)
 LOG_N = 20
 N_PAIRS = 1 << LOG_N
 MSMS_PER_STEP = 16  # commitments per step (one batch through spb_msm_batch*)
-N_SCALAR_SETS = 8   # 8 x 32 MiB of scalars rotate through the timed steps: 256 MiB > 126 MB L2
+N_SCALAR_SETS = 8   # 8 x 32 MiB of scalars rotate through the timed steps: 256 MiB > 50 MB L2
 R_MOD = 0x30644e72e131a029b85045b68181585d2833e84879b9709143e1f593f0000001
 STRONG_LOG_N = 23   # the north-star strong-scaling size: one 2^23 MSM on 1 GPU vs sharded over N
 SEED_POINTS, SEED_SCALARS = 0x5eed0002, 0x5eed0003
@@ -88,7 +93,7 @@ def measured_peaks():
     if os.path.exists(p):
         with open(p) as f:
             return json.load(f), "measured (MEASURED_PEAKS.json)"
-    return {"hbm_gbs": 6650.0}, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return {"hbm_gbs": 3350.0}, "H100 SXM data sheet (3.35 TB/s), not measured"
 
 
 class ClockSampler(threading.Thread):
@@ -127,7 +132,7 @@ def workload_config():
     """`config` of the JSON line: the WORKLOAD, identical in both arms (--impl ours / reference); how each arm runs it is in
     `schedule` (ours) / `cpu_baseline.sample` (reference)."""
     return {"workload": workload_text(), "log_n": LOG_N, "msms_per_step": MSMS_PER_STEP, "scalar_bits": 252,
-            "l2": "GPU arm: scalars rotate over 8 resident sets (256 MiB > 126 MB L2), the 64 MiB basis is reused as in the prover; "
+            "l2": "GPU arm: scalars rotate over 8 resident sets (256 MiB > 50 MB L2), the 64 MiB basis is reused as in the prover; "
                   "CPU arm: one scalar set, 96 MiB per MSM streams through the host caches"}
 
 
@@ -212,14 +217,11 @@ def main():
     ap.add_argument("--prove-k", type=int, default=23, help="k of the aggregation-shaped proof")
     ap.add_argument("--prove-k-step", type=int, default=20, help="k of the sync-step-shaped proof")
     ap.add_argument("--no-tables", action="store_true", help="skip spb_srs_precompute (W separate bucket sets, Horner over windows)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's commitments to DIR/msm_commitments_affine.npy")
     args = ap.parse_args()
     if args.warmup < 3 and args.impl == "ours":
         args.warmup = 3
     if args.impl == "reference":
-        if args.steps > 7:
-            args.steps = 7   # each step is a full 2^20 MSM on the CPU (0.3 - 1.5 s on the pool's hosts)
-        if args.steps < 5:
-            args.steps = 5
         return run_reference(args)
 
     import torch
@@ -314,6 +316,8 @@ def main():
     wall_ms = timed(run_dev, args.steps, args.warmup)
     launches = be.kernel_launches - launches0
     sampler.stop_flag = True; sampler.join(timeout=2)
+    if args.dump_outputs and rank == 0:
+        dump_commitments(args.dump_outputs, last["dev"][1])
     adds = be.last_msm_adds // MSMS_PER_STEP       # the counter accumulates over a batch
     stages_pipelined = be.last_msm_stage_ms         # last MSM of the timed batch (other lane running concurrently)
     e2e_steps = max(3, args.steps // 2)
@@ -467,25 +471,17 @@ def main():
     algo_bytes = 96.0 * N_PAIRS  # SURVEY.md 8d: 32 B scalar + 64 B affine base per pair, per launch (one rank's MSM)
     achieved = algo_bytes / (acc_ms * 1e-3) / 1e9 if acc_ms > 0 else None
     # INT32 multiply-pipe view: a mixed XYZZ addition = 7 products + 2 squarings + the lazily reduced pair; in units of the
-    # general product (measured peak 68 G/s) that is 9.25 (squaring 0.83, a*b-c*d 1.55: profiles/r02_field_ab.md)
+    # general product that is 9.25 (a squaring costs 0.83 of a product, a*b-c*d 1.55)
     modmul_per_launch = 9.25 * (adds - 2 * (1 if not args.no_tables else W) * (1 << (c - 1)))
-    traffic = None
-    tpath = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    if os.path.exists(tpath) and not args.no_tables:
-        with open(tpath) as f:
-            traffic = json.load(f)["msm_accumulate_kernel"]["dram_bytes_per_launch"]
     roofline = {
         "kernel": "msm_accumulate_kernel", "bound": "hbm", "achieved": achieved, "peak": peaks["hbm_gbs"], "unit": "GB/s",
-        "frac": (achieved / peaks["hbm_gbs"]) if achieved else None, "traffic": traffic, "peak_source": peak_src,
-        "traffic_source": "ncu --set full capture of this kernel (profiles/ncu_traffic.json names the commit it was taken at)",
+        "frac": (achieved / peaks["hbm_gbs"]) if achieved else None, "peak_source": peak_src,
         "algorithmic_bytes_per_launch": algo_bytes, "kernel_ms": acc_ms, "kernel_ms_in_timed_region_two_lanes_interleaved": acc_ms_overlapped,
         "kernel_share_of_msm": acc_ms / single_ms if single_ms else None,
         "note": "integer-ALU bound, not HBM bound (SURVEY.md finding 6): see int32_pipe",
         "int32_pipe": {"achieved_gmodmul_per_s": modmul_per_launch / (acc_ms * 1e-3) / 1e9 if acc_ms > 0 else None,
-                       "peak_gmodmul_per_s": 68.2, "peak_source": "tools/microbench.py modmul on this pool's B200 (profiles/r01_microbench.md)"},
+                       "peak_gmodmul_per_s": None, "peak_source": "not measured (tools/microbench.py modmul measures it)"},
     }
-    if roofline["int32_pipe"]["achieved_gmodmul_per_s"]:
-        roofline["int32_pipe"]["frac"] = roofline["int32_pipe"]["achieved_gmodmul_per_s"] / 68.2
 
     line = {
         "metric": "bn254_g1_msm_pairs_per_s", "value": value, "unit": "pairs/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
@@ -610,6 +606,18 @@ def main():
     be.close()
     if world > 1:
         dist.destroy_process_group()
+
+
+def dump_commitments(out_dir, points):
+    """(count, 12) Jacobian Montgomery limbs -> out_dir/msm_commitments_affine.npy, float64 (count, 2, 8): affine x, y as
+    little-endian 32-bit limbs (exact in float64; the affine form does not depend on the Jacobian representative)"""
+    from spectre_b200.halo2 import jacobian_to_affine_ints
+    out = np.empty((len(points), 2, 8), dtype=np.float64)
+    for i, p in enumerate(points):
+        for j, v in enumerate(jacobian_to_affine_ints(p)):
+            out[i, j] = [(v >> (32 * l)) & 0xFFFFFFFF for l in range(8)]
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "msm_commitments_affine.npy"), out)
 
 
 # ---- sections ---------------------------------------------------------------------------------------------------------------
@@ -747,8 +755,8 @@ def prove_both(torch, halo2, be, args):
                 E.sync(); t_py_host_rng = time.perf_counter() - t0
                 del E, pkey, srs
                 torch.cuda.empty_cache()
-                exe = cpp_driver.build_main_against_the_real_library()
-                with tempfile.TemporaryDirectory(dir="/tmp") as d:
+                with tempfile.TemporaryDirectory() as d:
+                    exe = cpp_driver.build_main_against_the_real_library(d)   # the tree may be read-only
                     head = "shape aggregation" if name == "aggregation_shape" else "shape halo2lib 15 2"
                     cpp_driver.dump_case(d, head, k, BENCH_VK_DIGEST, inst, copies, rec.counts, fixed_cols, adv_cols, rec.rows, secret, chacha_poly=host.chacha_seed)
                     rc, log, cproof, ms, kg = cpp_driver.run(exe, d, repeat=3, tables=True)

@@ -1,5 +1,5 @@
 /*
- * spectre_b200.h -- C ABI of libspectre_b200.so, the B200-native backend for the Halo2/KZG create_proof
+ * spectre_b200.h -- C ABI of libspectre_b200.so, the H100-native backend for the Halo2/KZG create_proof
  * hot path of ChainSafe/Spectre (MSM over BN254 G1, NTT over Fr, EvaluationDomain and batch polynomial ops).
  *
  * This is the drop-in boundary of SURVEY.md section 8b: exactly what a Rust `extern "C"` block in a
@@ -67,6 +67,10 @@ typedef struct spb_domain spb_domain; /* EvaluationDomain<Fr> constants */
  * what bench.py does. Returns NULL on failure (no CUDA device, bad id). */
 spb_ctx* spb_init(const int* device_ids, int n_dev);
 void spb_shutdown(spb_ctx* ctx);
+/* Free the context's cached device memory -- the grow-only workspaces of MSM, NTT and the provers, and the cached twiddle
+ * tables -- after the work queued on its devices is done; later calls allocate again as needed. For a long-lived context
+ * that ran large transforms before a proof that needs the memory. Fails while an spb_shplonk handle is open. */
+int spb_release_workspace(spb_ctx* ctx);
 const char* spb_last_error(spb_ctx* ctx);
 /* kernels launched by this context so far, and device milliseconds of the last timed call (CUDA events on the
  * context's own stream, taken inside every spb_msm* / spb_ntt* call). */
@@ -131,7 +135,8 @@ int spb_msm_batch(spb_ctx* ctx, const spb_srs* srs, int basis, const spb_fr* con
 int spb_msm_batch_dev(spb_ctx* ctx, const spb_srs* srs, int basis, const spb_fr* const* d_scalars, size_t n, size_t count, spb_g1* out);
 /* Precompute the 2^(c*j) multiples of the resident bases (W x the basis memory, one-time). Afterwards every MSM on
  * this SRS folds all windows into one bucket set with a wider window (fewer mixed additions, no window Horner).
- * Results are identical; only the schedule changes. */
+ * Results are identical; only the schedule changes. Tables that would take more than a quarter of a device's memory are
+ * not built (the call succeeds and the SRS keeps one bucket set per window). */
 int spb_srs_precompute(spb_ctx* ctx, spb_srs* srs);
 /* number of G1 additions (mixed + full) the last MSM executed on the device(s) */
 uint64_t spb_last_msm_adds(spb_ctx* ctx);

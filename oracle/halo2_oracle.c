@@ -5,7 +5,7 @@
  * path. Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs may
  * load this file's shared object; the product library (spectre_b200/csrc) never links or calls it.
  *
- * The arithmetic lives in third-party crates that are NOT vendored under /root/reference (no Cargo.lock,
+ * The arithmetic lives in third-party crates that are NOT vendored in the reference tree (no Cargo.lock,
  * no vendor dir -- SURVEY.md section 8c): halo2_proofs (PSE fork, pulled through halo2-base's `halo2-pse`
  * feature, reference Cargo.toml:44-48), halo2curves-axiom =0.5.2 (Cargo.toml:52), snark-verifier-sdk
  * v0.1.7-git (Cargo.toml:55-67), rand_chacha. Each function below names the upstream routine it

@@ -173,6 +173,7 @@ spb_ctx* spb_init(const int* device_ids, int n_dev) {
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, id) != cudaSuccess) { delete ctx; return nullptr; }
     d.sm_count = prop.multiProcessorCount;
+    d.total_mem = prop.totalGlobalMem;
     if (cudaStreamCreateWithFlags(&d.stream, cudaStreamNonBlocking) != cudaSuccess) { delete ctx; return nullptr; }
     cudaEventCreate(&d.ev0); cudaEventCreate(&d.ev1);
     cudaEventCreateWithFlags(&d.dep_ev, cudaEventDisableTiming);
@@ -213,6 +214,22 @@ void spb_shutdown(spb_ctx* ctx) {
     cudaStreamDestroy(d.stream);
   }
   delete ctx;
+}
+
+int spb_release_workspace(spb_ctx* ctx) {
+  if (!ctx) return SPB_ERR_ARG;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  if (ctx->shplonk_slots_busy) return set_error(ctx, SPB_ERR_STATE, "spb_release_workspace: an spb_shplonk handle is open");
+  for (auto& d : ctx->dev) {
+    SPB_CUDA(ctx, cudaSetDevice(d.device));
+    SPB_CUDA(ctx, cudaDeviceSynchronize());
+    for (auto& kv : d.slots) if (kv.second.ptr) cudaFree(kv.second.ptr);
+    d.slots.clear();
+    for (auto& t : d.ntt_tables) { cudaFree(t.tw_lo); cudaFree(t.tw_hi); if (t.tw_full) cudaFree(t.tw_full); }
+    d.ntt_tables.clear();
+  }
+  if (!ctx->dev.empty()) cudaSetDevice(ctx->dev[0].device);
+  return 0;
 }
 
 const char* spb_last_error(spb_ctx* ctx) { return ctx ? ctx->last_error.c_str() : "null context"; }

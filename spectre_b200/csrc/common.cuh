@@ -40,6 +40,7 @@ static const int kMaxMsmLanes = 4;
 struct DeviceState {
   int device = 0;
   int sm_count = 0;
+  size_t total_mem = 0;  // bytes of device memory
   cudaStream_t stream = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   cudaEvent_t dep_ev = nullptr;  // recorded on `stream` when other streams (MSM lanes, peer devices) must wait for it

@@ -179,10 +179,9 @@ template <class P> SPB_D Fp<P> fp_mul(const Fp<P>& A, const Fp<P>& B) {
 
 
 // ---- separate product and reduction: squaring, and a*b - c*d under one reduction -------------------------------------
-// Measured on B200 (profiles/r02_field_ab.md): the wide multiply-add (IMAD.WIDE = a fused mad.lo.cc / madc.hi.cc pair)
-// issues at 32 lanes/clk/SM and does NOT overlap with the integer adds around it -- their issue times add (an IADD3 costs
-// about 0.22 of an IMAD.WIDE). So the multiplier above (128 wide + ~60 other) is already at the optimum for a general
-// product: a Karatsuba split (48 + 64 wide, ~90 more adds) measured 1 % slower. What does pay is removing wide
+// The wide multiply-add (IMAD.WIDE = a fused mad.lo.cc / madc.hi.cc pair) does NOT overlap with the integer adds around it -- their issue times add (an IADD3 costs
+// a sizeable fraction of an IMAD.WIDE). So the multiplier above (128 wide + ~60 other) is already at the optimum for a general
+// product: a Karatsuba split (48 + 64 wide, ~90 more adds) trades wide multiplies for more adds than it saves. What does pay is removing wide
 // multiplies outright:
 //   * squaring: 28 cross products + 8 squares + 64 reduction rows = 100 wide instead of 128;
 //   * a*b - c*d (the y-coordinate of every XYZZ addition / doubling): two 64-wide products, ONE 64-wide reduction.

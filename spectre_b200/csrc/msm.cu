@@ -30,7 +30,7 @@ typedef MsmLane Lane;
 static const size_t kLanePinnedBytes = 256 * 1024;  // window partials of one MSM (<= 128 windows x a few points)
 static const int kMaxLanes = kMaxMsmLanes;
 // lanes a batch cycles through: 3 by default -- while one MSM accumulates, the latency-bound reduction tail of the previous one
-// and the sort of the next one fill the gaps (measured 2^20, ms per MSM: 1 lane 3.36, 2 lanes 2.95, 3 lanes 2.84); SPB_MSM_LANES=1..4
+// and the sort of the next one fill the gaps; SPB_MSM_LANES=1..4
 static int lane_count() {
   static int v = 0;
   if (!v) { const char* e = getenv("SPB_MSM_LANES"); v = e ? atoi(e) : 3; if (v < 1) v = 1; if (v > kMaxLanes) v = kMaxLanes; }
@@ -69,13 +69,12 @@ static void* lane_slot(spb_ctx* ctx, DeviceState& d, int lane, const char* name,
   return slot(ctx, d, buf, bytes);
 }
 
-// chunk length such that the accumulation grid is close to a whole number of waves (148 SMs x 512 resident threads)
+// chunk length such that the accumulation grid is close to a whole number of waves (sm_count SMs x 512 resident threads)
 static uint32_t choose_chunk(const DeviceState& d, uint64_t est_entries) {
   if (const char* e = getenv("SPB_MSM_CHUNK")) { int v = atoi(e); if (v >= 8 && v <= 256) return (uint32_t)v; }
   const double wave = (double)d.sm_count * 512.0;
-  // entry lists of 2^24 and more (2^21 pairs with tables): the chunk pieces (two 128-byte points per chunk) no longer fit the L2 and
-  // the stitch pass becomes DRAM-latency bound -- 2^22 pairs: 1.79 ms at L = 32, 0.31 ms at L = 96 for +0.14 ms of accumulation
-  // (profiles/r02_msm_probe.md); with hundreds of waves the tail of the last wave does not matter
+  // long entry lists: the chunk pieces (two 128-byte points per chunk, 8 B per entry at L = 32) no longer fit the L2 and the
+  // stitch pass becomes DRAM-latency bound; with hundreds of waves the tail of the last wave does not matter
   if (est_entries >= kLongChunkMinEntries) return kLongChunk;
   double waves = (double)est_entries / 32.0 / wave;
   if (waves < 1.0) return 32;
@@ -135,7 +134,7 @@ static int msm_enqueue(spb_ctx* ctx, DeviceState& d, int lane, Lane& ln, const F
   SPB_CUDA(ctx, cudaMemcpyAsync(counts, offsets, (nb + 1) * 4, cudaMemcpyDeviceToDevice, st));
   cudaEventRecord(ln.ev[2], st);
   // (Two alternatives to this one-pass counting sort were built and measured slower at every size -- a second scatter pass with
-  // L2-resident write windows, and a bin-local sort ranking in shared memory: profiles/r02_msm_probe.md.)
+  // L2-resident write windows, and a bin-local sort ranking in shared memory.)
   msm_scatter_kernel<<<(unsigned)((n + tb - 1) / tb), tb, 0, st>>>(n, d_scalars, g, counts, ent);
   const uint32_t* total = offsets + nb;  // number of entries M, resident on the device
   cudaEventRecord(ln.ev[3], st);
@@ -566,7 +565,14 @@ static int msm_batch_common(spb_ctx* ctx, const spb_srs* srs, int basis, const s
   if (!ctx || !srs || !out || (count && !scalars)) return SPB_ERR_ARG;
   std::lock_guard<std::mutex> lk(ctx->mu);
   ctx->last_msm_adds = 0;
-  const size_t NL = (size_t)lane_count();
+  // every lane holds a workspace sized for these MSMs (sorted entries, chunk pieces, buckets); lanes beyond the first are
+  // used only while their workspaces together stay within a tenth of the device's memory (H100, 80 GB: three lanes for a
+  // K = 23 SRS with tables, one for K = 24 without), so a large proof keeps its memory for its polynomials
+  const MsmGeom lg = srs->table_c ? msm_make_geometry(srs->table_c, true, 0) : msm_choose_geometry(n ? n : 1);
+  const uint64_t ents = (uint64_t)n * lg.W;
+  const uint64_t lane_bytes = ents * sizeof(MsmEntry) + 2 * (ents / kShortChunk + 1) * (sizeof(G1Xyzz) + 4) + (uint64_t)lg.BW * lg.B * sizeof(G1Xyzz);
+  const uint64_t fit = ctx->dev[0].total_mem / 10 / (lane_bytes ? lane_bytes : 1);
+  const size_t NL = std::max<size_t>(1, std::min<size_t>((size_t)lane_count(), (size_t)fit));
   std::vector<MsmPart> jobs[kMaxLanes];
   for (size_t i = 0; i < count; i++) {
     int lane = (int)(i % NL);
@@ -607,6 +613,17 @@ int spb_srs_precompute(spb_ctx* ctx, spb_srs* srs) {
   size_t per_dev = srs->shards.empty() ? srs->n : srs->shards[0].count;
   uint32_t c = msm_choose_c(per_dev ? per_dev : 1, true);
   uint32_t W = (255 + c - 1) / c;
+  // The tables are built only while they take at most a quarter of each device's memory: on an 80 GB H100 that keeps them
+  // for both bases of a K = 23 SRS (12 GiB) but not of K = 24 (24 GiB), which would leave too little for the proof's
+  // polynomials. Without tables the SRS keeps one bucket set per window; results are the same either way.
+  for (auto& sh : srs->shards) {
+    if (!sh.count) continue;
+    SPB_CUDA(ctx, cudaSetDevice(ctx->dev[sh.dev_index].device));
+    size_t free_b = 0, total_b = 0;
+    SPB_CUDA(ctx, cudaMemGetInfo(&free_b, &total_b));
+    const size_t bases = (sh.g ? 1 : 0) + (sh.g_lagrange ? 1 : 0);
+    if ((size_t)W * sh.count * sizeof(G1Affine) * bases > total_b / 4) return 0;
+  }
   for (auto& sh : srs->shards) {
     if (!sh.count) continue;
     DeviceState& d = ctx->dev[sh.dev_index];

@@ -1,4 +1,4 @@
-// BN254 G1 multi-scalar multiplication for sm_100a: signed-digit windowed Pippenger with a
+// BN254 G1 multi-scalar multiplication for sm_90a: signed-digit windowed Pippenger with a
 // counting sort and a load-balanced segmented bucket accumulation.
 //
 // Replaces halo2_proofs::arithmetic::best_multiexp / multiexp_serial ([UPSTREAM] halo2_proofs/src/arithmetic.rs;
@@ -21,8 +21,8 @@
 //                 a chunk ("tail") and the run that enters one ("head") are stored as chunk pieces.
 //   5. stitch   : one thread per tail piece walks the following head pieces of the same key and stores the
 //                 bucket; chains longer than a cap (giant buckets) go to block-wide / grid-wide tree reductions.
-//                 (Summing the pieces inside the group reduction of step 6 instead was measured: -0.2 ms of stitch, +0.3 ms of
-//                 groups at 2^20 -- three adder sites in one thread either cost 255 registers or an out-of-line adder.)
+//                 (Summing the pieces inside the group reduction of step 6 instead costs more in the groups than it saves in
+//                 the stitch -- three adder sites in one thread either cost 255 registers or an out-of-line adder.)
 //   6. reduce   : per bucket set S = sum_b (b+1) * bucket[b]: groups of 8 buckets by a running sum per thread, then the group
 //                 sums viewed as an R x C matrix: sum_t t*S1_t = C * sum_r r*Row_r + sum_c c*Col_c -- tree sums and local
 //                 weights < 2^7 only.
@@ -57,7 +57,9 @@ struct alignas(8) MsmEntry { uint32_t key, val; };
 // digits -- so every kernel that cuts the list derives the same effective length from the entry count on the device.
 static const uint32_t kLongChunk = 96, kShortChunk = 32;
 #ifndef SPB_LONG_CHUNK_MIN_ENTRIES
-#define SPB_LONG_CHUNK_MIN_ENTRIES (1ull << 24)   // tests/hostemu lowers it to run the long-chunk path on CPU-sized inputs
+// 2^23 entries = 64 MB of short-chunk pieces, beyond H100's 50 MB L2; tests/hostemu lowers it to run the long-chunk path on
+// CPU-sized inputs
+#define SPB_LONG_CHUNK_MIN_ENTRIES (1ull << 23)
 #endif
 static const uint64_t kLongChunkMinEntries = SPB_LONG_CHUNK_MIN_ENTRIES;
 SPB_HD uint32_t msm_effective_chunk(uint32_t L, uint64_t M) { return (L == kLongChunk && M < kLongChunkMinEntries) ? kShortChunk : L; }
@@ -320,8 +322,8 @@ inline G1Xyzz msm_tail_finish(const MsmGeom& g, const G1Xyzz* part) {
 // (witness columns are full of repeated small values) are found with match.any and served by ONE atomic, so a column
 // of equal scalars costs one atomic per warp and window instead of 32 serialised ones on the same address. The loop
 // is kept convergent (inactive lanes carry a flag instead of leaving) so the warp-level primitives are well defined.
-// Lanes of the warp holding the same key as the caller (inactive lanes pass kNoKey). MATCH.ANY costs ~80 issue cycles per warp on
-// sm_100a and was what bound the histogram and sort kernels (ncu: top stall of msm_count / msm_bin_local_sort), while only columns
+// Lanes of the warp holding the same key as the caller (inactive lanes pass kNoKey). MATCH.ANY costs tens of issue cycles per warp
+// and was what bound the histogram and sort kernels (ncu: top stall of msm_count / msm_bin_local_sort), while only columns
 // of repeated values need the grouping -- and those show equal keys in NEIGHBOURING lanes. So: one shuffle + vote decide; without
 // neighbouring duplicates every lane is its own group (any duplicates elsewhere in the warp just take their own atomics, which is
 // always correct -- the grouping is an optimisation).
@@ -416,7 +418,7 @@ __device__ void block_sum2_xyzz(G1Xyzz& a, G1Xyzz& b, G1Xyzz* sh /* NT entries *
 // kHugeChain links (a column of equal scalars puts n/32 pieces into one bucket) are handed on to the huge-chain
 // kernels, which spread ONE chain over the whole grid.
 static const uint32_t kHugeChain = 4096;
-static const uint32_t kHugeBlocks = 1184;   // 8 CTAs of 128 threads per SM on 148 SMs
+static const uint32_t kHugeBlocks = 1056;   // 8 CTAs of 128 threads per SM on 132 SMs (H100 SXM)
 __global__ void __launch_bounds__(128) msm_giant_kernel(const uint32_t* total, uint32_t L, const uint32_t* giant_count, const uint32_t* giant_list,
                                                         const uint32_t* head_key, const G1Xyzz* head, const uint32_t* tail_key, const G1Xyzz* tail,
                                                         G1Xyzz* buckets, uint32_t* huge_count, uint32_t* huge_list /* pairs: t0, end */) {

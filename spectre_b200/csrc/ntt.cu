@@ -8,8 +8,8 @@
 namespace spb {
 
 // log2 elements per shared-memory tile. 2^11 elements (~68 KB of limb planes + twiddles) with 256 threads lets two
-// CTAs share an SM, so one tile's global load/store phases overlap the other's butterflies: measured 8-15 % faster
-// than one 2^12-element CTA per SM (profiles/r01_bench_progress.md, NTT knob sweep); 2^10 is best up to 2^20.
+// CTAs share an SM (H100: 227 KB of shared memory per block, 228 KB per SM), so one tile's global load/store phases overlap
+// the other's butterflies; 2^10 up to 2^20.
 static uint32_t g_tile_log_override = 0;
 static uint32_t tile_elems_log(uint32_t k) {
   static bool init = false;
@@ -83,7 +83,7 @@ static int launch_pass(spb_ctx* ctx, DeviceState& d, const NttPlan& plan, uint32
   // persistent CTAs: as many as fit the SMs (shared memory bound), striding over the tiles
   uint64_t per_sm = (227 * 1024) / (L.smem + 1024); if (per_sm < 1) per_sm = 1; if (per_sm > 4) per_sm = 4;
   uint64_t grid = (uint64_t)d.sm_count * per_sm; if (grid > L.tiles) grid = L.tiles;
-  // Measured (profiles/r01_bench_progress.md): persistence pays up to 2^20 (launch + twiddle staging amortised); beyond
+  // Persistence pays up to 2^20 (launch + twiddle staging amortised); beyond
   // that co-resident persistent CTAs run their load/compute phases in lockstep and lose the overlap that
   // hardware-scheduled one-tile CTAs get for free, so large transforms launch one CTA per tile.
   if (k > 20) grid = L.tiles;

@@ -1,4 +1,4 @@
-// Fr number-theoretic transform for sm_100a: multi-pass (four-step / six-step family) decimation-in-frequency
+// Fr number-theoretic transform for sm_90a: multi-pass (four-step / six-step family) decimation-in-frequency
 // NTT with shared-memory tiles, radix-4 register butterflies and shared-memory twiddle staging.
 //
 // Replaces halo2_proofs::arithmetic::best_fft ([UPSTREAM] halo2_proofs/src/arithmetic.rs; reached from the

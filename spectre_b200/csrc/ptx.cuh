@@ -1,4 +1,4 @@
-// Carry-chain primitives for 256-bit modular arithmetic on sm_100a.
+// Carry-chain primitives for 256-bit modular arithmetic on sm_90a.
 //
 // On the device every function is exactly one (or one fused pair of) PTX instruction(s) that reads or
 // writes the implicit carry flag CC.CF. ptxas fuses a `mad.lo.cc` / `madc.hi.cc` pair on an adjacent

@@ -107,6 +107,10 @@ class Backend:
         if rc != 0:
             raise BackendError("%s failed (%d): %s" % (what, rc, self.lib.spb_last_error(self.ctx).decode()))
 
+    def release_workspace(self):
+        """spb_release_workspace: free the cached workspaces and twiddle tables of every device"""
+        self.check(self.lib.spb_release_workspace(self.ctx), "spb_release_workspace")
+
     def stream(self, dev_index=0):
         """cudaStream_t (int) every `_dev` call of that device is ordered on: enqueue the producers of device buffers there."""
         self.lib.spb_stream.restype = ctypes.c_void_p
@@ -352,7 +356,7 @@ class Backend:
         self.check(self.lib.spb_test_field_op(self.ctx, f, o, _p(a), _p(b), _p(out), ctypes.c_size_t(a.shape[0])), "spb_test_field_op")
         return out
 
-    def bench_modmul(self, field="fq", threads=148 * 2048, iters=2000, ilp=2):
+    def bench_modmul(self, field="fq", threads=132 * 2048, iters=2000, ilp=2):
         ms = ctypes.c_float(0)
         self.check(self.lib.spb_bench_modmul(self.ctx, {"fr": 0, "fq": 1}[field], ctypes.c_uint32(threads), ctypes.c_uint32(iters), ilp, ctypes.byref(ms)), "spb_bench_modmul")
         threads = (threads + 255) // 256 * 256
@@ -366,7 +370,7 @@ class Backend:
                                                  ctypes.byref(ms), ctypes.byref(adds)), "spb_bench_accumulate")
         return ms.value, adds.value / (ms.value * 1e-3)
 
-    def bench_pipe(self, kind, threads=148 * 2048, iters=4000):
+    def bench_pipe(self, kind, threads=132 * 2048, iters=4000):
         """-> (ms, instructions of the probed kind per second; for interleaved kinds: pairs per second)"""
         ms = ctypes.c_float(0)
         self.check(self.lib.spb_bench_pipe(self.ctx, kind, ctypes.c_uint32(threads), ctypes.c_uint32(iters), ctypes.byref(ms)), "spb_bench_pipe")

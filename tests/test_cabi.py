@@ -1,4 +1,4 @@
-"""CPU-only: the C-ABI library builds for sm_100a, loads, exports every symbol include/spectre_b200.h declares,
+"""CPU-only: the C-ABI library builds for sm_90a, loads, exports every symbol include/spectre_b200.h declares,
 and refuses to run without a GPU (no CPU fallback). No compute calls here."""
 import ctypes
 import os
@@ -58,9 +58,9 @@ def test_only_abi_symbols_are_exported(libpath):
     assert exported and all(s.startswith("spb_") for s in exported), exported
 
 
-def test_cubin_is_sm_100a(libpath):
+def test_cubin_is_sm_90a(libpath):
     out = subprocess.run(["cuobjdump", "-lelf", libpath], capture_output=True, text=True).stdout
-    assert "sm_100a" in out
+    assert "sm_90a" in out
 
 
 def test_no_cpu_fallback_without_gpu(libpath):

@@ -33,7 +33,7 @@ def main():
     counts = [bf + 1, 1, bf + 1, bf + 1, 2, bf, 1, bf, 1, n, 1, cs.degree() - 1]
     rng = SeededRng(fx["seed"])
     exe = _build_shim_and_main()
-    with tempfile.TemporaryDirectory(dir="/tmp") as d:
+    with tempfile.TemporaryDirectory() as d:
         with open(os.path.join(d, "meta.txt"), "w") as f:
             f.write("shape aggregation\nk %d\ndigest %x\ninstances %s\n" % (k, int(fx["vk_digest"]), " ".join("%x" % v for v in instances)))
             for (c1, r1), (c2, r2) in copies:

@@ -3,12 +3,12 @@
 verifier contract): a proof of the aggregation-shaped synthetic circuit at K = 23
 (the size the reference's sync_step verifier contract is generated for), made by the proof driver bound to the CPU
 ORACLE, then replayed through the reference's own verifier contract (tests/yul_harness.py) -- the fixture is only
-written if the contract accepts it. Build-container only (needs /root/reference and ~25 GiB of RAM, ~10 minutes).
+written if the contract accepts it. Needs the reference's contracts/snark-verifiers and ~25 GiB of RAM (~10 minutes).
 
 The GPU test tests/test_gpu_plonk.py::test_k23_proof_equals_the_contract_accepted_fixture regenerates the same proof
 with the CUDA engine (same seed, same witness) and requires identical bytes.
 
-usage: python tools/make_k23_fixture.py [--k 23] [--check-only]
+usage: python tools/make_k23_fixture.py --contracts <reference checkout>/contracts/snark-verifiers [--k 23]
 """
 import argparse
 import json
@@ -55,6 +55,7 @@ def inputs(k, kats):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--k", type=int, default=23)
+    ap.add_argument("--contracts", required=True, help="the reference's contracts/snark-verifiers directory")
     args = ap.parse_args()
     with open(os.path.join(GOLDEN, "verifier_kats.json")) as f:
         kats = json.load(f)
@@ -70,13 +71,11 @@ def main():
     proof = plonk.create_proof(E, pk, [instances], [adv], SeededRng(SEED), T, timings)
     print("proof %.1fs" % (time.time() - t0), {a: round(b, 1) for a, b in timings.items()}, flush=True)
     vk_points = pk.fixed_commitments + pk.sigma_commitments
-    with open("/tmp/k%d_candidate.json" % k, "w") as f:      # kept for debugging a rejection without re-proving
-        json.dump({"instances": [hex(v) for v in instances], "vk_points": [[hex(x), hex(y)] for x, y in vk_points], "proof": proof.hex()}, f)
     if k in CONTRACTS:
         contract, _, kat = CONTRACTS[k]
         want = tuple(int(v, 16) for v in kats[kat]["xy"])
         assert pk.fixed_commitments[1] == want, "range-table commitment differs from the contract's VK constant"
-        ok, m = yul_harness.run_contract(contract, instances, proof, vk_points, tau, kats)
+        ok, m = yul_harness.run_contract(args.contracts, contract, instances, proof, vk_points, tau, kats)
         print("contract accepted:", ok, m.precompile_counts, flush=True)
         assert ok and m.pairing_calls == 1, "the reference verifier contract rejected the proof"
         fixture = {"_source": "tools/make_k23_fixture.py --k %d: proof driver on the CPU oracle; accepted by contracts/snark-verifiers/%s.sol replayed by tests/yul_harness.py" % (k, contract),
