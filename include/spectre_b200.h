@@ -128,7 +128,7 @@ int spb_msm(spb_ctx* ctx, const spb_srs* srs, int basis, const spb_fr* scalars, 
 /* same with the scalars already resident on device 0 of the context */
 int spb_msm_dev(spb_ctx* ctx, const spb_srs* srs, int basis, const spb_fr* d_scalars, size_t n, spb_g1* out);
 /* `count` MSMs of n scalars each against the same resident basis (create_proof commits its advice / permutation /
- * lookup columns back to back against g_lagrange). Consecutive MSMs cycle over three stream lanes (SPB_MSM_LANES) so the
+ * lookup columns back to back against g_lagrange). Consecutive MSMs cycle over three stream lanes so the
  * latency-bound tail of one and the sort of the next overlap the accumulation of the one in between; out[i] belongs to
  * scalars[i]. */
 int spb_msm_batch(spb_ctx* ctx, const spb_srs* srs, int basis, const spb_fr* const* scalars, size_t n, size_t count, spb_g1* out);
@@ -318,14 +318,6 @@ int spb_test_field_op(spb_ctx* ctx, int field, int op, const spb_fr* a, const sp
 /* modular-multiply throughput microbenchmark: `iters` dependent products per thread over `threads` threads, `ilp`
  * independent chains each (1, 2 or 4; ilp | 0x100 = two chains of squarings); returns device milliseconds in *ms. */
 int spb_bench_modmul(spb_ctx* ctx, int field, uint32_t threads, uint32_t iters, int ilp, float* ms);
-/* Accumulation probe: every thread keeps K running sums and adds `rounds` points (gathered at pseudo-random indices from a table
- * of 2^table_log distinct points, like the MSM's sorted entries) to each. mode 0 = XYZZ mixed additions (the product's
- * schedule), mode 1 = batched affine additions sharing one inversion per thread and round (state in global memory).
- * Returns device milliseconds and the number of point additions. A throughput experiment, not a product path. */
-int spb_bench_accumulate(spb_ctx* ctx, int mode, uint32_t threads, uint32_t K, uint32_t rounds, uint32_t table_log, float* ms, uint64_t* additions);
-/* raw issue-rate probe of one pipe (8 independent chains per thread, `iters` x 8 instructions each):
- * kind 0 IMAD.WIDE, 1 IMAD, 2 DFMA, 3 IMAD.WIDE+DFMA interleaved, 4 IADD, 5 IMAD.WIDE+IADD interleaved. */
-int spb_bench_pipe(spb_ctx* ctx, int kind, uint32_t threads, uint32_t iters, float* ms);
 
 #if defined(__GNUC__)
 #pragma GCC visibility pop

@@ -35,6 +35,26 @@ void* slot(spb_ctx* ctx, DeviceState& d, const char* name, size_t bytes) {
   return b.ptr;
 }
 
+// Below these sizes a pass is launch-bound and stays on the first device. The environment may lower them (SPB_SHARD_MIN_ROWS,
+// SPB_SHARD_MIN_LOGN) so that a small circuit runs the multi-device paths; read on every call, as a test sets them at run time.
+static uint64_t shard_threshold(const char* var, uint64_t dflt, uint64_t least) {
+  const char* e = getenv(var);
+  const long long v = e ? atoll(e) : 0;
+  return v >= (long long)least ? (uint64_t)v : dflt;
+}
+
+std::vector<RowRange> row_ranges(spb_ctx* ctx, uint64_t rows) {
+  const size_t D = ctx->dev.size();
+  if (D < 2 || !ctx->peer_access || rows < shard_threshold("SPB_SHARD_MIN_ROWS", (uint64_t)1 << 16, 256)) return {RowRange{0, 0, rows}};
+  std::vector<RowRange> v;
+  const uint64_t per = ((rows + D - 1) / D + 255) / 256 * 256;
+  for (size_t i = 0; i < D; i++) {
+    const uint64_t lo = per * i, hi = lo + per < rows ? lo + per : rows;
+    if (lo < hi) v.push_back(RowRange{(int)i, lo, hi});
+  }
+  return v;
+}
+
 // Double-buffered staging: two pinned 16 MiB buffers per device (slot-like, allocated once). While the DMA of one buffer is
 // in flight (cudaMemcpyAsync + an event), the host fills / drains the other, so the file system and the PCIe copy overlap
 // instead of alternating as a synchronous cudaMemcpy loop does. (cuFile / GDS would remove the bounce buffer altogether; the
@@ -123,32 +143,6 @@ __global__ void modmul_bench_kernel(Fp<P>* out, uint32_t iters) {
   Fp<P> acc = x[0];
 #pragma unroll
   for (int j = 1; j < ILP; j++) acc = fp_add(acc, x[j]);
-  out[tid] = acc;
-}
-
-// Raw pipe-rate probes (8 independent chains per thread): 0 = IMAD.WIDE.U32, 1 = IMAD (lo), 2 = DFMA,
-// 3 = IMAD.WIDE + DFMA interleaved 1:1, 4 = IADD3, 5 = IMAD.WIDE + IADD3 interleaved 1:1
-template <int KIND>
-__global__ void pipe_probe_kernel(unsigned long long* out, uint32_t iters, uint32_t seed) {
-  uint32_t tid = blockIdx.x * blockDim.x + threadIdx.x;
-  unsigned long long w[8]; uint32_t v[8]; double f[8];
-  uint32_t a = tid * 2654435761u + seed, b = a ^ 0x9e3779b9u;
-  double fa = 1.0 + (double)(tid & 1023) * 1e-9, fb = 0.999999 + (double)(seed & 7) * 1e-9;
-#pragma unroll
-  for (int j = 0; j < 8; j++) { w[j] = a + j; v[j] = b + j; f[j] = fa + j; }
-  for (uint32_t i = 0; i < iters; i++) {
-#pragma unroll
-    for (int j = 0; j < 8; j++) {
-      // one multiplicand is the chain's own low word so the product is not loop-invariant
-      if (KIND == 0 || KIND == 3 || KIND == 5) asm volatile("{ .reg .u32 lo, hi; mov.b64 {lo, hi}, %0; mad.wide.u32 %0, lo, %1, %0; }" : "+l"(w[j]) : "r"(b));
-      if (KIND == 1) asm volatile("mad.lo.u32 %0, %0, %1, %2;" : "+r"(v[j]) : "r"(a), "r"(b));
-      if (KIND == 2 || KIND == 3) asm volatile("fma.rz.f64 %0, %0, %1, %2;" : "+d"(f[j]) : "d"(fb), "d"(fa));
-      if (KIND == 4 || KIND == 5) asm volatile("add.u32 %0, %0, %1;" : "+r"(v[j]) : "r"(b));
-    }
-  }
-  unsigned long long acc = 0;
-#pragma unroll
-  for (int j = 0; j < 8; j++) acc += w[j] + v[j] + (unsigned long long)__double_as_longlong(f[j]);
   out[tid] = acc;
 }
 
@@ -487,9 +481,7 @@ int spb_extended_to_coeff_dev(spb_ctx* ctx, const spb_domain* dm, const spb_fr* 
 // pass's output through NVLink peer access, intermediate passes run in their own HBM.
 static int ntt_batch_devices(spb_ctx* ctx, const spb_fr* const* d_in, spb_fr* const* d_out, size_t count, uint32_t k, const Fr& omega, const NttOpts& o) {
   DeviceState& d0 = ctx->dev[0];
-  uint32_t min_k = 16;   // smaller transforms are launch-bound: first device only (tests lower it: SPB_SHARD_MIN_LOGN)
-  if (const char* e = getenv("SPB_SHARD_MIN_LOGN")) { int v = atoi(e); if (v >= 1) min_k = (uint32_t)v; }
-  const size_t D = (ctx->peer_access && ctx->dev.size() > 1 && k >= min_k) ? ctx->dev.size() : 1;
+  const size_t D = (ctx->peer_access && ctx->dev.size() > 1 && k >= shard_threshold("SPB_SHARD_MIN_LOGN", 16, 1)) ? ctx->dev.size() : 1;
   SPB_CUDA(ctx, cudaSetDevice(d0.device));
   SPB_CUDA(ctx, cudaEventRecord(d0.ev0, d0.stream));
   if (D > 1) SPB_CUDA(ctx, cudaEventRecord(d0.dep_ev, d0.stream));
@@ -550,32 +542,6 @@ int spb_test_field_op(spb_ctx* ctx, int field, int op, const spb_fr* a, const sp
   ctx->n_kernel_launches++;
   SPB_CUDA(ctx, cudaMemcpyAsync(out, buf + 2 * n, n * 32, cudaMemcpyDeviceToHost, d.stream));
   SPB_CUDA(ctx, cudaStreamSynchronize(d.stream));
-  return 0;
-}
-
-int spb_bench_pipe(spb_ctx* ctx, int kind, uint32_t threads, uint32_t iters, float* ms) {
-  if (!ctx || !ms) return SPB_ERR_ARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  DeviceState& d = ctx->dev[0];
-  SPB_CUDA(ctx, cudaSetDevice(d.device));
-  threads = (threads + 255) / 256 * 256;
-  unsigned long long* buf = (unsigned long long*)slot(ctx, d, "test_io", (size_t)threads * 8);
-  if (!buf) return SPB_ERR_OOM;
-  unsigned blocks = threads / 256;
-  SPB_CUDA(ctx, cudaEventRecord(d.ev0, d.stream));
-  switch (kind) {
-    case 0: pipe_probe_kernel<0><<<blocks, 256, 0, d.stream>>>(buf, iters, 1); break;
-    case 1: pipe_probe_kernel<1><<<blocks, 256, 0, d.stream>>>(buf, iters, 1); break;
-    case 2: pipe_probe_kernel<2><<<blocks, 256, 0, d.stream>>>(buf, iters, 1); break;
-    case 3: pipe_probe_kernel<3><<<blocks, 256, 0, d.stream>>>(buf, iters, 1); break;
-    case 4: pipe_probe_kernel<4><<<blocks, 256, 0, d.stream>>>(buf, iters, 1); break;
-    default: pipe_probe_kernel<5><<<blocks, 256, 0, d.stream>>>(buf, iters, 1); break;
-  }
-  SPB_CUDA(ctx, cudaGetLastError());
-  ctx->n_kernel_launches++;
-  SPB_CUDA(ctx, cudaEventRecord(d.ev1, d.stream));
-  SPB_CUDA(ctx, cudaStreamSynchronize(d.stream));
-  SPB_CUDA(ctx, cudaEventElapsedTime(ms, d.ev0, d.ev1));
   return 0;
 }
 

@@ -35,7 +35,9 @@ struct MsmLane {
   void* pinned = nullptr;
   bool ready = false;
 };
-static const int kMaxMsmLanes = 4;
+// Lanes a batch cycles through: while one MSM accumulates, the latency-bound reduction tail of the previous one and the sort of
+// the next one fill the gaps.
+static const int kMaxMsmLanes = 3;
 
 struct DeviceState {
   int device = 0;
@@ -85,6 +87,12 @@ void* slot(spb_ctx* ctx, DeviceState& d, const char* name, size_t bytes);
     int rc_ = (expr);            \
     if (rc_ != 0) return rc_;    \
   } while (0)
+
+// ---- capi.cu: multi-device sharding of one pass ----
+// Row ranges of a pass over `rows` rows, one per device, starting at multiples of 256 rows; a single range on the first device
+// when the context has one device, no peer access, or the pass is short enough to be launch-bound.
+struct RowRange { int dev_index; uint64_t lo, hi; };
+std::vector<RowRange> row_ranges(spb_ctx* ctx, uint64_t rows);
 
 // ---- capi.cu: file <-> device streaming through two pinned staging buffers (read of chunk i+1 overlaps the DMA of chunk i) ----
 int stream_file_to_device(spb_ctx* ctx, DeviceState& d, FILE* f, void* d_dst, size_t bytes, const char* what);

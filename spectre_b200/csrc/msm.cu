@@ -28,14 +28,6 @@ namespace spb {
 // The lanes of a device (common.cuh: MsmLane) live in its DeviceState, i.e. in the context: nothing here is process-wide.
 typedef MsmLane Lane;
 static const size_t kLanePinnedBytes = 256 * 1024;  // window partials of one MSM (<= 128 windows x a few points)
-static const int kMaxLanes = kMaxMsmLanes;
-// lanes a batch cycles through: 3 by default -- while one MSM accumulates, the latency-bound reduction tail of the previous one
-// and the sort of the next one fill the gaps; SPB_MSM_LANES=1..4
-static int lane_count() {
-  static int v = 0;
-  if (!v) { const char* e = getenv("SPB_MSM_LANES"); v = e ? atoi(e) : 3; if (v < 1) v = 1; if (v > kMaxLanes) v = kMaxLanes; }
-  return v;
-}
 // call with the context lock held (every entry point that runs an MSM holds it)
 static int get_lane(spb_ctx* ctx, int dev_index, int lane_index, Lane** out) {
   Lane& l = ctx->dev[dev_index].lanes[lane_index];
@@ -71,7 +63,6 @@ static void* lane_slot(spb_ctx* ctx, DeviceState& d, int lane, const char* name,
 
 // chunk length such that the accumulation grid is close to a whole number of waves (sm_count SMs x 512 resident threads)
 static uint32_t choose_chunk(const DeviceState& d, uint64_t est_entries) {
-  if (const char* e = getenv("SPB_MSM_CHUNK")) { int v = atoi(e); if (v >= 8 && v <= 256) return (uint32_t)v; }
   const double wave = (double)d.sm_count * 512.0;
   // long entry lists: the chunk pieces (two 128-byte points per chunk, 8 B per entry at L = 32) no longer fit the L2 and the
   // stitch pass becomes DRAM-latency bound; with hundreds of waves the tail of the last wave does not matter
@@ -572,8 +563,8 @@ static int msm_batch_common(spb_ctx* ctx, const spb_srs* srs, int basis, const s
   const uint64_t ents = (uint64_t)n * lg.W;
   const uint64_t lane_bytes = ents * sizeof(MsmEntry) + 2 * (ents / kShortChunk + 1) * (sizeof(G1Xyzz) + 4) + (uint64_t)lg.BW * lg.B * sizeof(G1Xyzz);
   const uint64_t fit = ctx->dev[0].total_mem / 10 / (lane_bytes ? lane_bytes : 1);
-  const size_t NL = std::max<size_t>(1, std::min<size_t>((size_t)lane_count(), (size_t)fit));
-  std::vector<MsmPart> jobs[kMaxLanes];
+  const size_t NL = std::max<size_t>(1, std::min<size_t>((size_t)kMaxMsmLanes, (size_t)fit));
+  std::vector<MsmPart> jobs[kMaxMsmLanes];
   for (size_t i = 0; i < count; i++) {
     int lane = (int)(i % NL);
     if (i >= NL) SPB_TRY(job_collect(ctx, lane, jobs[lane], &out[i - NL]));  // MSM i-NL ran on this lane
@@ -645,81 +636,6 @@ int spb_srs_precompute(spb_ctx* ctx, spb_srs* srs) {
     }
   }
   srs->table_c = c;
-  return 0;
-}
-
-// ---- accumulation micro-benchmark (VERDICT r1 item 3b: an experiment, not an estimate) -------------------------------------
-// Both kernels add `rounds` gathered affine points to every one of K running sums per thread, the points read from a table
-// at pseudo-random indices as the MSM's sorted entries do.
-//   mode 0: XYZZ mixed additions, the K sums visited one after the other (sum in registers while its `rounds` points arrive).
-//   mode 1: batched affine additions: per round the K pending additions of a thread share ONE inversion (Montgomery's trick):
-//           forward pass d_j = x_P - x_acc, prefix products to memory; Fermat inversion of the total; backward pass
-//           lambda = (y_P - y_acc) / d_j, x3 = lambda^2 - x_acc - x_P, y3 = lambda (x_acc - x3) - y_acc. Sums and prefix
-//           products live in global memory laid out [j][thread] (coalesced). Exceptional cases (equal x) cannot occur for the
-//           random table other than with negligible probability and are not handled: this is a throughput probe, not a product path.
-static __device__ __forceinline__ uint32_t bench_index(uint32_t tid, uint32_t j, uint32_t r, uint32_t mask) {
-  uint32_t h = tid * 2654435761u ^ (j * 40503u + r * 2246822519u);
-  h ^= h >> 15; h *= 2246822519u; h ^= h >> 13;
-  return h & mask;
-}
-__global__ void __launch_bounds__(128) bench_acc_xyzz_kernel(const G1Affine* table, uint32_t mask, uint32_t K, uint32_t rounds, G1Xyzz* out) {
-  const uint32_t tid = blockIdx.x * blockDim.x + threadIdx.x, nthreads = gridDim.x * blockDim.x;
-  for (uint32_t j = 0; j < K; j++) {
-    G1Xyzz acc = xyzz_from_affine(msm_load_point(table, bench_index(tid, j, 0xffffu, mask)));
-    for (uint32_t r = 0; r < rounds; r++) xyzz_add_mixed(acc, msm_load_point(table, bench_index(tid, j, r, mask)));
-    out[(uint64_t)j * nthreads + tid] = acc;
-  }
-}
-__global__ void __launch_bounds__(128) bench_acc_affine_kernel(const G1Affine* table, uint32_t mask, uint32_t K, uint32_t rounds, G1Affine* sums, Fq* prefix) {
-  const uint32_t tid = blockIdx.x * blockDim.x + threadIdx.x, nthreads = gridDim.x * blockDim.x;
-  for (uint32_t j = 0; j < K; j++) sums[(uint64_t)j * nthreads + tid] = msm_load_point(table, bench_index(tid, j, 0xffffu, mask));
-  for (uint32_t r = 0; r < rounds; r++) {
-    Fq run = fp_one<FqParams>();
-    for (uint32_t j = 0; j < K; j++) {
-      const Fq ax = sums[(uint64_t)j * nthreads + tid].x;
-      const Fq px = table[bench_index(tid, j, r, mask)].x;
-      prefix[(uint64_t)j * nthreads + tid] = run;                       // product of the denominators before j
-      run = fp_mul(run, fp_sub(px, ax));
-    }
-    Fq inv = fp_inv(run);
-    for (int j = (int)K - 1; j >= 0; j--) {
-      const G1Affine a = sums[(uint64_t)j * nthreads + tid];
-      const G1Affine p = msm_load_point(table, bench_index(tid, (uint32_t)j, r, mask));
-      const Fq d = fp_sub(p.x, a.x);
-      const Fq dinv = fp_mul(inv, prefix[(uint64_t)j * nthreads + tid]);
-      inv = fp_mul(inv, d);
-      const Fq lambda = fp_mul(fp_sub(p.y, a.y), dinv);
-      G1Affine s;
-      s.x = fp_sub(fp_sub(fp_sqr(lambda), a.x), p.x);
-      s.y = fp_sub(fp_mul(lambda, fp_sub(a.x, s.x)), a.y);
-      sums[(uint64_t)j * nthreads + tid] = s;
-    }
-  }
-}
-
-int spb_bench_accumulate(spb_ctx* ctx, int mode, uint32_t threads, uint32_t K, uint32_t rounds, uint32_t table_log, float* ms, uint64_t* additions) {
-  if (!ctx || !ms || !K || !rounds || table_log < 4 || table_log > 24) return SPB_ERR_ARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  DeviceState& d = ctx->dev[0];
-  SPB_CUDA(ctx, cudaSetDevice(d.device));
-  threads = (threads + 127) / 128 * 128;
-  const uint64_t tn = 1ull << table_log;
-  Fr* sc = (Fr*)slot(ctx, d, "srs_scalars", tn * sizeof(Fr));
-  G1Affine* table = (G1Affine*)slot(ctx, d, "bacc_table", tn * sizeof(G1Affine));
-  G1Xyzz* out = (G1Xyzz*)slot(ctx, d, "bacc_state", (uint64_t)threads * K * sizeof(G1Xyzz));      // XYZZ sums, or affine sums + prefix products
-  if (!sc || !table || !out) return SPB_ERR_OOM;
-  Fr g; { constexpr uint32_t v[8] = SPB_FR_DELTA_MONT; for (int i = 0; i < 8; i++) g.l[i] = v[i]; }
-  srs_scalars_kernel<<<(unsigned)((tn + 127) / 128), 128, 0, d.stream>>>(0, g, g, g, 1, tn, sc);       // table[i] = delta^(i+1) * G1: distinct points
-  g1_fixed_base_mul_kernel<<<(unsigned)((tn + 127) / 128), 128, 0, d.stream>>>(sc, tn, table);
-  SPB_CUDA(ctx, cudaEventRecord(d.ev0, d.stream));
-  if (mode == 0) bench_acc_xyzz_kernel<<<threads / 128, 128, 0, d.stream>>>(table, (uint32_t)(tn - 1), K, rounds, out);
-  else bench_acc_affine_kernel<<<threads / 128, 128, 0, d.stream>>>(table, (uint32_t)(tn - 1), K, rounds, (G1Affine*)out, (Fq*)((G1Affine*)out + (uint64_t)threads * K));
-  SPB_CUDA(ctx, cudaGetLastError());
-  ctx->n_kernel_launches += 3;
-  SPB_CUDA(ctx, cudaEventRecord(d.ev1, d.stream));
-  SPB_CUDA(ctx, cudaStreamSynchronize(d.stream));
-  SPB_CUDA(ctx, cudaEventElapsedTime(ms, d.ev0, d.ev1));
-  if (additions) *additions = (uint64_t)threads * K * rounds;
   return 0;
 }
 

@@ -636,7 +636,6 @@ inline MsmGeom msm_make_geometry(uint32_t c, bool precomp, uint32_t tab_stride) 
 //   10 * n * W  (mixed additions)  +  2 * 14 * BW * 2^(c-1)  (running sums over the buckets, full additions)
 // BW = W without precomputed tables, 1 with them (all windows share one bucket set).
 inline uint32_t msm_choose_c(uint64_t n, bool precomp) {
-  if (const char* e = getenv(precomp ? "SPB_MSM_C_TABLES" : "SPB_MSM_C")) { int v = atoi(e); if (v >= 3 && v <= 22) return (uint32_t)v; }
   uint32_t best = 0; double best_cost = 0;
   for (uint32_t c = 3; c <= 22; c++) {
     uint32_t W = (255 + c - 1) / c;

@@ -2,7 +2,6 @@
 #define SPB_NTT_KERNELS 1
 #include "common.cuh"
 #include "ntt.cuh"
-#include <stdlib.h>
 #include <string.h>
 
 namespace spb {
@@ -10,27 +9,15 @@ namespace spb {
 // log2 elements per shared-memory tile. 2^11 elements (~68 KB of limb planes + twiddles) with 256 threads lets two
 // CTAs share an SM (H100: 227 KB of shared memory per block, 228 KB per SM), so one tile's global load/store phases overlap
 // the other's butterflies; 2^10 up to 2^20.
-static uint32_t g_tile_log_override = 0;
-static uint32_t tile_elems_log(uint32_t k) {
-  static bool init = false;
-  if (!init) { const char* e = getenv("SPB_NTT_TILE_LOG"); if (e) { g_tile_log_override = (uint32_t)atoi(e); if (g_tile_log_override < 6) g_tile_log_override = 6; if (g_tile_log_override > 12) g_tile_log_override = 12; } init = true; }
-  if (g_tile_log_override) return g_tile_log_override;
-  return k <= 20 ? 10 : 11;
-}
+static uint32_t tile_elems_log(uint32_t k) { return k <= 20 ? 10 : 11; }
 // largest sub-NTT held in one shared-memory tile (11: two passes up to 2^22; the tile is then 2048 x 2 columns)
-static uint32_t max_digit_bits() {
-  static uint32_t v = 0;
-  if (!v) { const char* e = getenv("SPB_NTT_MAX_DIGIT"); v = e ? (uint32_t)atoi(e) : 11; if (v < 4) v = 4; if (v > 12) v = 12; }
-  return v;
-}
+static const uint32_t kMaxDigitBits = 11;
+// threads per pass CTA
+static const uint32_t kPassThreads = 256;
 // full omega^i tables are kept while their total stays under this many bytes per device (else two-level tables)
-static size_t full_table_budget() {
-  static size_t v = 0;
-  if (!v) { const char* e = getenv("SPB_NTT_FULL_TABLE_MB"); v = (e ? (size_t)atoll(e) : 6144) << 20; if (!v) v = 1; }
-  return v;
-}
+static const size_t kFullTableBudget = (size_t)6 << 30;
 
-static NttPlan make_plan(uint32_t k) { return ntt_make_plan(k, max_digit_bits()); }
+static NttPlan make_plan(uint32_t k) { return ntt_make_plan(k, kMaxDigitBits); }
 
 static int get_tables(spb_ctx* ctx, DeviceState& d, uint32_t k, const Fr& omega, uint32_t h, NttTables** out) {
   for (auto& t : d.ntt_tables)
@@ -47,7 +34,7 @@ static int get_tables(spb_ctx* ctx, DeviceState& d, uint32_t k, const Fr& omega,
     size_t used = 0;
     for (auto& o : d.ntt_tables) if (o.tw_full) used += ((size_t)1 << o.k) * sizeof(Fr);
     size_t need = ((size_t)1 << k) * sizeof(Fr);
-    if (k >= 12 && used + need <= full_table_budget() && cudaMalloc(&t.tw_full, need) == cudaSuccess) {
+    if (k >= 12 && used + need <= kFullTableBudget && cudaMalloc(&t.tw_full, need) == cudaSuccess) {
       fr_pow_table_kernel<<<(unsigned)((((size_t)1 << k) + 127) / 128), 128, 0, d.stream>>>(t.tw_full, omega, (uint64_t)1 << k, 0);
       ctx->n_kernel_launches++;
     } else {
@@ -66,19 +53,13 @@ static int get_tables(spb_ctx* ctx, DeviceState& d, uint32_t k, const Fr& omega,
   return 0;
 }
 
-static uint32_t max_threads_per_cta() {
-  static uint32_t v = 0;
-  if (!v) { const char* e = getenv("SPB_NTT_THREADS"); v = e ? (uint32_t)atoi(e) : 256; if (v < 32 || v > 512) v = 512; }
-  return v;
-}
-
 // Geometry of pass `pi` (ntt_fill_pass, shared with the host emulation) and its launch.
 static int launch_pass(spb_ctx* ctx, DeviceState& d, const NttPlan& plan, uint32_t pi, uint32_t k, const NttTables* tb, uint32_t h,
                        const Fr* src, Fr* dst, const NttOpts& opts, const NttShare& sh) {
   NttPassParams p;
   p.src = src; p.dst = dst; p.tw_lo = tb->tw_lo; p.tw_hi = tb->tw_hi; p.tw_full = tb->tw_full;
   NttOptsHost oh; oh.n_in = opts.n_in; oh.n_out = opts.n_out; oh.pre3 = opts.pre3; oh.post3 = opts.post3;
-  NttLaunch L = ntt_fill_pass(p, plan, pi, k, h, oh, sh, tile_elems_log(k), max_threads_per_cta());
+  NttLaunch L = ntt_fill_pass(p, plan, pi, k, h, oh, sh, tile_elems_log(k), kPassThreads);
   if (L.smem > 227 * 1024) return set_error(ctx, SPB_ERR_STATE, "ntt: tile needs %zu B of shared memory", L.smem);
   // persistent CTAs: as many as fit the SMs (shared memory bound), striding over the tiles
   uint64_t per_sm = (227 * 1024) / (L.smem + 1024); if (per_sm < 1) per_sm = 1; if (per_sm > 4) per_sm = 4;
@@ -128,7 +109,6 @@ int ntt_device(spb_ctx* ctx, DeviceState& d, const Fr* d_src, Fr* d_dst, uint32_
 bool ntt_multi_applicable(spb_ctx* ctx, uint32_t k) {
   size_t G = ctx->dev.size();
   if (G < 2 || (G & (G - 1))) return false;
-  if (getenv("SPB_NTT_SINGLE_DEVICE")) return false;
   if (k < 16) return false;
   NttPlan plan = make_plan(k);
   uint32_t g = 0; while ((1u << g) < G) g++;
@@ -220,15 +200,6 @@ int ntt_multi_host(spb_ctx* ctx, const Fr* in, Fr* out, uint32_t k, const Fr& om
     SPB_CUDA(ctx, cudaStreamSynchronize(d.stream));
     float ms = 0.f; cudaEventElapsedTime(&ms, d.ev0, d.ev1);
     if (ms > worst) worst = ms;
-  }
-  if (getenv("SPB_NTT_MD_DEBUG")) {
-    for (size_t q = 0; q < G; q++) {
-      DeviceState& d = ctx->dev[q];
-      cudaSetDevice(d.device);
-      float a = 0, b = 0, c = 0;
-      cudaEventElapsedTime(&a, d.ev0, d.stage_ev[0]); cudaEventElapsedTime(&b, d.stage_ev[0], d.stage_ev[1]); cudaEventElapsedTime(&c, d.stage_ev[1], d.ev1);
-      fprintf(stderr, "[spb ntt md] k=%u dev %zu: pass1 %.3f ms, all-to-all (incl. wait) %.3f ms, remaining passes %.3f ms, peer_access=%d\n", k, q, a, b, c, (int)ctx->peer_access);
-    }
   }
   if (ev_ms) *ev_ms = worst;
   ctx->last_kernel_ms = worst;

@@ -11,14 +11,8 @@
 #include "common.cuh"
 #include "quotient.cuh"
 #include <string.h>
-#include <chrono>
-#include <stdlib.h>
 
 using namespace spb;
-
-// SPB_PLONK_DEBUG=1: wall-clock of the SHPLONK phases on stderr
-static bool plonk_debug() { static int v = -1; if (v < 0) { const char* e = getenv("SPB_PLONK_DEBUG"); v = e && *e && *e != '0'; } return v == 1; }
-static double now_s() { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
 
 namespace {
 
@@ -78,24 +72,6 @@ __global__ void sub_small_kernel(Fr* a, SmallPoly s) {
 
 namespace {
 
-// Row ranges of one grand-product column over the devices of the context (SURVEY.md 8e "grand product ... one all-gather of G
-// partial products + local fix-up"): multiples of 256 rows, one range per device; a single range when the context has one device,
-// no peer access, or the column is short (launch-bound; tests lower the threshold with SPB_SHARD_MIN_ROWS).
-struct ProdRange { int dev_index; size_t lo, hi; };
-std::vector<ProdRange> product_ranges(spb_ctx* ctx, size_t n) {
-  std::vector<ProdRange> v;
-  const size_t D = ctx->dev.size();
-  size_t min_rows = (size_t)1 << 16;
-  if (const char* e = getenv("SPB_SHARD_MIN_ROWS")) { long long m = atoll(e); if (m >= 256) min_rows = (size_t)m; }
-  if (D > 1 && ctx->peer_access && n >= min_rows) {
-    const size_t per = ((n + D - 1) / D + 255) / 256 * 256;
-    for (size_t i = 0; i < D; i++) { size_t lo = per * i, hi = lo + per < n ? lo + per : n; if (lo < hi) v.push_back(ProdRange{(int)i, lo, hi}); }
-  } else {
-    v.push_back(ProdRange{0, 0, n});
-  }
-  return v;
-}
-
 // z[0] = init, z[i+1] = z[i] * num[i] / den[i] over the n rows of one column, then the last n_blinds entries <- blinds and
 // *tail_out <- z[n - n_blinds - 1] (synchronises). `terms(d, lo, cnt, num, den)` enqueues on d.stream the kernel that writes the
 // cnt numerators / denominators of rows lo.. into the device-local buffers.
@@ -106,7 +82,7 @@ std::vector<ProdRange> product_ranges(spb_ctx* ctx, size_t n) {
 template <class Terms>
 int fraction_product(spb_ctx* ctx, size_t n, const Terms& terms, const Fr& init, const spb_fr* blinds, uint32_t n_blinds, Fr* dz, Fr* tail_out) {
   DeviceState& d0 = ctx->dev[0];
-  const std::vector<ProdRange> ranges = product_ranges(ctx, n);
+  const std::vector<RowRange> ranges = row_ranges(ctx, n);
   const size_t G = ranges.size();
   std::vector<Fr*> nums(G, nullptr), dtot(G, nullptr);
   if (G > 1) { SPB_CUDA(ctx, cudaSetDevice(d0.device)); SPB_CUDA(ctx, cudaEventRecord(d0.dep_ev, d0.stream)); }   // the caller's inputs are ordered on d0.stream
@@ -299,7 +275,6 @@ int spb_shplonk_begin_dev(spb_ctx* ctx, const spb_srs* srs, size_t n, const spb_
   if (!ctx) return SPB_ERR_ARG;
   if (!srs || !sets || !n_sets || !y || !v || !h_commitment || !out || n < 2) return set_error(ctx, SPB_ERR_ARG, "spb_shplonk_begin_dev: null argument");
   *out = nullptr;
-  const double t_start = now_s();
   uint32_t total = 0;
   for (uint32_t i = 0; i < n_sets; i++) {
     const spb_rotation_set& rs = sets[i];
@@ -309,7 +284,6 @@ int spb_shplonk_begin_dev(spb_ctx* ctx, const spb_srs* srs, size_t n, const spb_
   }
   spb_shplonk* s = new spb_shplonk();
   s->ctx = ctx; s->n = n; s->srs = srs; s->n_polys = total; s->y = fr_load(y); s->v = fr_load(v);
-  const double t_alloc = now_s();
   // host side: the sets, the low-degree equivalents R_ij and the super point set
   std::vector<const Fr*> ptrs; ptrs.reserve(total);
   for (uint32_t i = 0; i < n_sets; i++) {
@@ -390,9 +364,7 @@ int spb_shplonk_begin_dev(spb_ctx* ctx, const spb_srs* srs, size_t n, const spb_
     }
     SHP_CUDA(cudaGetLastError());
   }
-  const double t_polys = now_s();
   rc = spb_msm_dev(ctx, srs, SPB_BASIS_G, (const spb_fr*)s->d_h, n, h_commitment);
-  if (plonk_debug()) fprintf(stderr, "[spb] shplonk begin n=%zu polys=%u: alloc %.1f ms, quotients %.1f ms, msm %.1f ms\n", n, total, (t_alloc - t_start) * 1e3, (t_polys - t_alloc) * 1e3, (now_s() - t_polys) * 1e3);
   if (rc != 0) { std::lock_guard<std::mutex> lk(ctx->mu); shplonk_release(s); return rc; }
   *out = s;
   return 0;
@@ -403,7 +375,6 @@ int spb_shplonk_finish_dev(spb_ctx* ctx, spb_shplonk* s, const spb_fr* u, spb_g1
   if (!s || !u || !commitment) return set_error(ctx, SPB_ERR_ARG, "spb_shplonk_finish_dev: null argument");
   const Fr uu = fr_load(u);
   const size_t n = s->n;
-  const double t_start = now_s();
   const uint32_t n_sets = (uint32_t)s->sets.size();
   // weights w_ij = v^i * Z_{T \ S_i}(u) * y^j; constant = sum w_ij * R_ij(u); and -Z_T(u) on h
   std::vector<Fr> w; w.reserve(s->n_polys);
@@ -451,11 +422,8 @@ int spb_shplonk_finish_dev(spb_ctx* ctx, spb_shplonk* s, const spb_fr* u, spb_g1
     SHP_CUDA(cudaGetLastError());
     SHP_CUDA(cudaStreamSynchronize(d.stream));
   }
-  const double t_polys = now_s();
   rc = spb_msm_dev(ctx, s->srs, SPB_BASIS_G, (const spb_fr*)s->d_tmp[1], n - 1, commitment);
-  const double t_msm = now_s();
   { std::lock_guard<std::mutex> lk(ctx->mu); shplonk_release(s); }
-  if (plonk_debug()) fprintf(stderr, "[spb] shplonk finish: linearisation %.1f ms, msm %.1f ms, release %.1f ms\n", (t_polys - t_start) * 1e3, (t_msm - t_polys) * 1e3, (now_s() - t_msm) * 1e3);
   return rc;
 }
 

@@ -13,7 +13,6 @@
 // not pinned by any reference-owned vector (none exists for this row).
 #include "common.cuh"
 #include "quotient.cuh"
-#include <stdlib.h>
 #include <string.h>
 #include <algorithm>
 #include <utility>
@@ -44,29 +43,13 @@ __global__ void __launch_bounds__(256) lookup_constraints_kernel(LookupArgs a) {
 
 namespace {
 
-// Row-range shards of one pass over `size` extended rows (SURVEY.md 8e "evaluate_h / pointwise": embarrassingly parallel by
-// extended-row range). The polynomials stay where the caller put them -- on the first device of the context; the other
-// devices run the same kernel on their row range and read the inputs (rotations included: any row of any polynomial) and
-// write their slice of `values` straight through NVLink peer access, so no halo is exchanged and no staging copy exists.
-struct RowShard { int dev_index; uint64_t lo, hi; };
-std::vector<RowShard> row_shards(spb_ctx* ctx, uint64_t size) {
-  std::vector<RowShard> v;
-  const size_t D = ctx->dev.size();
-  uint64_t min_rows = (uint64_t)1 << 16;   // below this a pass is launch-bound: one device (tests lower it: SPB_SHARD_MIN_ROWS)
-  if (const char* e = getenv("SPB_SHARD_MIN_ROWS")) { long long v = atoll(e); if (v >= 256) min_rows = (uint64_t)v; }
-  if (D > 1 && ctx->peer_access && size >= min_rows) {
-    const uint64_t per = ((size + D - 1) / D + 255) / 256 * 256;
-    for (size_t i = 0; i < D; i++) {
-      uint64_t lo = per * i, hi = lo + per < size ? lo + per : size;
-      if (lo < hi) v.push_back(RowShard{(int)i, lo, hi});
-    }
-  } else {
-    v.push_back(RowShard{0, 0, size});
-  }
-  return v;
-}
-// the shard's device: current device set, its stream ordered after everything queued on the first device's stream so far
-int shard_begin(spb_ctx* ctx, const RowShard& sh) {
+// Each pass runs in row-range shards over `size` extended rows (row_ranges; SURVEY.md 8e "evaluate_h / pointwise":
+// embarrassingly parallel by extended-row range). The polynomials stay where the caller put them -- on the first device of the
+// context; the other devices run the same kernel on their row range and read the inputs (rotations included: any row of any
+// polynomial) and write their slice of `values` straight through NVLink peer access, so no halo is exchanged and no staging
+// copy exists.
+// shard_begin: the shard's device is made current, its stream ordered after everything queued on the first device's stream so far
+int shard_begin(spb_ctx* ctx, const RowRange& sh) {
   DeviceState& d0 = ctx->dev[0];
   DeviceState& d = ctx->dev[sh.dev_index];
   SPB_CUDA(ctx, cudaSetDevice(d.device));
@@ -76,7 +59,7 @@ int shard_begin(spb_ctx* ctx, const RowShard& sh) {
   return 0;
 }
 // wait for every shard; last_kernel_ms = device time of the pass on the first device's clock
-int shards_finish(spb_ctx* ctx, const std::vector<RowShard>& shards) {
+int shards_finish(spb_ctx* ctx, const std::vector<RowRange>& shards) {
   DeviceState& d0 = ctx->dev[0];
   for (auto& sh : shards) {
     if (sh.dev_index == 0) continue;
@@ -217,7 +200,7 @@ int spb_graph_evaluate_dev(spb_ctx* ctx, const spb_graph* g, const spb_fr* const
   uint32_t n_inter = g->num_intermediates, n_calc = g->num_calculations;
   const uint32_t* prog = g->program;
   size_t prog_n = g->program_words;
-  if (g->program_words && !getenv("SPB_GRAPH_NO_SCHEDULE") && schedule_program(g->program, g->program_words, g->num_calculations, prog_words, n_inter, n_calc)) {
+  if (g->program_words && schedule_program(g->program, g->program_words, g->num_calculations, prog_words, n_inter, n_calc)) {
     prog = prog_words.data(); prog_n = prog_words.size();
   } else {
     n_inter = g->num_intermediates; n_calc = g->num_calculations;
@@ -226,7 +209,7 @@ int spb_graph_evaluate_dev(spb_ctx* ctx, const spb_graph* g, const spb_fr* const
   std::vector<Fr> sc(4 + n_challenges);
   memcpy(&sc[0], beta, 32); memcpy(&sc[1], gamma, 32); memcpy(&sc[2], theta, 32); memcpy(&sc[3], y, 32);
   if (n_challenges) memcpy(&sc[4], challenges, (size_t)n_challenges * 32);
-  const std::vector<RowShard> shards = row_shards(ctx, size);
+  const std::vector<RowRange> shards = row_ranges(ctx, size);
   for (auto& sh : shards) {
     DeviceState& d = ctx->dev[sh.dev_index];
     SPB_TRY(shard_begin(ctx, sh));
@@ -288,7 +271,7 @@ int spb_permutation_constraints_dev(spb_ctx* ctx, spb_fr* d_values, uint64_t siz
   std::vector<Fr> pw(256);
   pw[0] = fp_one<FrParams>();
   for (int j = 1; j < 256; j++) pw[j] = fp_mul(pw[j - 1], a.extended_omega);
-  const std::vector<RowShard> shards = row_shards(ctx, size);
+  const std::vector<RowRange> shards = row_ranges(ctx, size);
   for (auto& sh : shards) {
     DeviceState& d = ctx->dev[sh.dev_index];
     SPB_TRY(shard_begin(ctx, sh));
@@ -318,7 +301,7 @@ int spb_lookup_constraints_dev(spb_ctx* ctx, spb_fr* d_values, uint64_t size, in
   a.product = (const Fr*)d_product; a.permuted_input = (const Fr*)d_permuted_input; a.permuted_table = (const Fr*)d_permuted_table;
   a.table_value = (const Fr*)d_table_value; a.l0 = (const Fr*)d_l0; a.l_last = (const Fr*)d_l_last; a.l_active = (const Fr*)d_l_active;
   memcpy(&a.beta, beta, 32); memcpy(&a.gamma, gamma, 32); memcpy(&a.y, y, 32);
-  const std::vector<RowShard> shards = row_shards(ctx, size);
+  const std::vector<RowRange> shards = row_ranges(ctx, size);
   for (auto& sh : shards) {
     DeviceState& d = ctx->dev[sh.dev_index];
     SPB_TRY(shard_begin(ctx, sh));

@@ -363,21 +363,6 @@ class Backend:
         return ms.value, threads * iters * (2 if ilp & 0x100 else ilp) / (ms.value * 1e-3)
 
 
-    def bench_accumulate(self, mode, threads, K, rounds, table_log=20):
-        """-> (ms, point additions per second); mode 0 XYZZ mixed additions, 1 batched affine (one inversion per thread and round)"""
-        ms = ctypes.c_float(0); adds = ctypes.c_uint64(0)
-        self.check(self.lib.spb_bench_accumulate(self.ctx, ctypes.c_int(mode), ctypes.c_uint32(threads), ctypes.c_uint32(K), ctypes.c_uint32(rounds), ctypes.c_uint32(table_log),
-                                                 ctypes.byref(ms), ctypes.byref(adds)), "spb_bench_accumulate")
-        return ms.value, adds.value / (ms.value * 1e-3)
-
-    def bench_pipe(self, kind, threads=132 * 2048, iters=4000):
-        """-> (ms, instructions of the probed kind per second; for interleaved kinds: pairs per second)"""
-        ms = ctypes.c_float(0)
-        self.check(self.lib.spb_bench_pipe(self.ctx, kind, ctypes.c_uint32(threads), ctypes.c_uint32(iters), ctypes.byref(ms)), "spb_bench_pipe")
-        threads = (threads + 255) // 256 * 256
-        return ms.value, threads * iters * 8 / (ms.value * 1e-3)
-
-
 class EvaluationDomain:
     """EvaluationDomain::<Fr>::new(j, k) ([UPSTREAM] halo2_proofs/src/poly/domain.rs)."""
 

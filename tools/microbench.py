@@ -40,26 +40,6 @@ def main():
                     ms, rate = be.bench_modmul(field, sms * tpsm, 2000, ilp)
                     print(json.dumps({"bench": "modmul", "op": nm, "field": field, "threads_per_sm": tpsm, "ms": round(ms, 3), "gop_per_s": round(rate / 1e9, 2),
                                       "lib": os.path.basename(halo2.LIB_PATH)}), flush=True)
-    if "accumulate" in what:
-        # XYZZ mixed additions vs batched affine additions with K pending additions per thread sharing one inversion
-        for tpsm in (512,):
-            be.bench_accumulate(0, sms * tpsm, 4, 8)
-            ms, rate = be.bench_accumulate(0, sms * tpsm, 8, 32)
-            print(json.dumps({"bench": "accumulate", "schedule": "xyzz_mixed", "threads_per_sm": tpsm, "K": 8, "rounds": 32, "ms": round(ms, 3), "gadds_per_s": round(rate / 1e9, 3)}), flush=True)
-        for tpsm in (256, 512):
-            for K in (16, 32, 64, 128, 256, 512):
-                rounds = max(2, 2048 // K)
-                be.bench_accumulate(1, sms * tpsm, K, 1)
-                ms, rate = be.bench_accumulate(1, sms * tpsm, K, rounds)
-                print(json.dumps({"bench": "accumulate", "schedule": "batched_affine", "threads_per_sm": tpsm, "K": K, "rounds": rounds, "ms": round(ms, 3),
-                                  "gadds_per_s": round(rate / 1e9, 3)}), flush=True)
-    if "pipe" in what:
-        names = {0: "IMAD.WIDE.U32", 1: "IMAD", 2: "DFMA", 3: "IMAD.WIDE+DFMA (pairs)", 4: "IADD", 5: "IMAD.WIDE+IADD (pairs)"}
-        for kind in range(6):
-            be.bench_pipe(kind, sms * 2048, 500)
-            ms, rate = be.bench_pipe(kind, sms * 2048, 4000)
-            print(json.dumps({"bench": "pipe", "kind": names[kind], "ms": round(ms, 3), "tera_inst_per_s": round(rate / 1e12, 3),
-                              "lanes_per_clk_per_sm_at_1.9GHz": round(rate / sms / 1.9e9, 1)}), flush=True)
     if "ntt" in what:
         import torch
         root = pow(7, (R_MOD - 1) >> 28, R_MOD)

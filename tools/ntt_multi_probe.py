@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""In-process multi-device NTT timing probe (set SPB_NTT_MD_DEBUG=1 for the per-phase split)."""
+"""In-process multi-device NTT timing probe: wall clock and device time of spb_ntt over every visible GPU."""
 import ctypes, os, sys, time
 import numpy as np, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
-"""Development probe (GPU box): create_proof of one circuit shape a few times with per-stage wall clock; with
-SPB_PLONK_DEBUG=1 the library prints the SHPLONK phases. usage: prove_probe.py [aggregation|halo2lib] [k] [reps]"""
+"""Development probe (GPU box): create_proof of one circuit shape a few times with per-stage wall clock.
+usage: prove_probe.py [aggregation|halo2lib] [k] [reps]"""
 import json
 import os
 import sys
