@@ -56,6 +56,7 @@ typedef struct spb_domain spb_domain; /* EvaluationDomain<Fr> constants */
 #define SPB_ERR_OOM (-3)
 #define SPB_ERR_STATE (-4)
 #define SPB_ERR_CONSTRAINT (-5) /* halo2's Error::ConstraintSystemFailure (lookup input not in table) */
+#define SPB_ERR_DATA (-6)       /* invalid input data: halo2's io::ErrorKind::InvalidData */
 
 #define SPB_BASIS_G 0          /* monomial basis  (Params::commit)          */
 #define SPB_BASIS_G_LAGRANGE 1 /* Lagrange basis  (Params::commit_lagrange) */
@@ -106,9 +107,20 @@ void spb_srs_free(spb_ctx* ctx, spb_srs* srs);
  * (g_to_lagrange: the inverse DFT over the group, on the device; no knowledge of the secret needed). The reference keeps
  * a degree -> params map for exactly this (prover/src/prover.rs:34). Returns a NEW handle without window tables. */
 int spb_srs_downsize(spb_ctx* ctx, const spb_srs* srs, uint32_t k, spb_srs** out);
-/* ParamsKZG::read / ::write, SerdeFormat::RawBytes: k (u32 LE) | g[2^k] | g_lagrange[2^k] | g2 | s_g2 with every
- * coordinate as its in-memory Montgomery limbs -- the `params/kzg_bn254_{k}.srs` file halo2-base's gen_srs caches
- * (reference: prover/src/cli.rs:48, .gitignore:36). Read streams the points straight into device memory. */
+/* ParamsKZG::read_custom / ::write: k (u32 LE) | g[2^k] | g_lagrange[2^k] | g2 | s_g2 with every coordinate as its
+ * in-memory Montgomery limbs -- the `params/kzg_bn254_{k}.srs` file halo2-base's gen_srs caches (reference:
+ * prover/src/cli.rs:48, .gitignore:36). The read streams the points straight into device memory.
+ *   SPB_SERDE_RAW_BYTES: the checked format (upstream's ParamsKZG::read). Every coordinate's stored limbs must be less than
+ *     p and every point must lie on its curve (G1: y^2 = x^3 + 3; G2: y^2 = x^3 + 3/(9+u)) or be the identity (0, 0). The
+ *     G1 points are checked on the device that holds them, the G2 trailer on the host. Otherwise the call returns
+ *     SPB_ERR_DATA and the error text names the first invalid point in file order (g, g_lagrange, g2, s_g2) and the
+ *     reason, e.g. "g_lagrange[262144]: not on the curve". spb_last_device_ms then gives the check kernels' device time.
+ *   SPB_SERDE_RAW_BYTES_UNCHECKED: no checks.
+ * Any other format is SPB_ERR_ARG (the compressed SerdeFormat::Processed is not implemented). On failure *out is untouched. */
+#define SPB_SERDE_RAW_BYTES 1
+#define SPB_SERDE_RAW_BYTES_UNCHECKED 2
+int spb_srs_read_file_custom(spb_ctx* ctx, const char* path, int format, spb_srs** out);
+/* spb_srs_read_file_custom(.., SPB_SERDE_RAW_BYTES_UNCHECKED, ..): does NOT validate the points */
 int spb_srs_read_file(spb_ctx* ctx, const char* path, spb_srs** out);
 int spb_srs_write_file(spb_ctx* ctx, const spb_srs* srs, const char* path);
 int spb_srs_set_g2(spb_ctx* ctx, spb_srs* srs, const unsigned char g2[128], const unsigned char s_g2[128]);

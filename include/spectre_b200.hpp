@@ -7,7 +7,7 @@
 //   halo2::arithmetic::best_multiexp(coeffs, bases) -> G1      (panics -> std::invalid_argument on length mismatch)
 //   halo2::arithmetic::best_fft(a, omega, log_n)               (in place; a.size() must be 1 << log_n)
 //   halo2::poly::EvaluationDomain(j, k)                        lagrange_to_coeff / coeff_to_extended / ...
-//   halo2::poly::kzg::ParamsKZG                                from_parts / setup / commit / commit_lagrange
+//   halo2::poly::kzg::ParamsKZG                                from_parts / setup / read_custom / commit / commit_lagrange
 //
 // Header-only; link with -lspectre_b200. There is no CPU fallback: Backend() throws when spb_init fails.
 #pragma once
@@ -131,6 +131,13 @@ class ParamsKZG {
     spb_srs* h = nullptr;
     be.check(spb_srs_setup(be.ctx(), k, &s, &h), "spb_srs_setup");
     return ParamsKZG(be, k, h);
+  }
+  // ParamsKZG::read_custom(reader, format) of a params file: format SPB_SERDE_RAW_BYTES (checked: canonical coordinates, every
+  // point on its curve; throws naming the first invalid point) or SPB_SERDE_RAW_BYTES_UNCHECKED
+  static ParamsKZG read_custom(const Backend& be, const std::string& path, int format) {
+    spb_srs* h = nullptr;
+    be.check(spb_srs_read_file_custom(be.ctx(), path.c_str(), format, &h), "spb_srs_read_file_custom");
+    return ParamsKZG(be, spb_srs_k(h), h);
   }
   ParamsKZG(ParamsKZG&& o) noexcept : be_(o.be_), k_(o.k_), h_(o.h_) { o.h_ = nullptr; }
   ~ParamsKZG() { if (h_) spb_srs_free(be_.ctx(), h_); }

@@ -58,6 +58,9 @@ pub struct spb_rotation_set {
 pub const SPB_BASIS_G: c_int = 0;
 pub const SPB_BASIS_G_LAGRANGE: c_int = 1;
 pub const SPB_ERR_CONSTRAINT: c_int = -5;
+pub const SPB_ERR_DATA: c_int = -6;
+pub const SPB_SERDE_RAW_BYTES: c_int = 1;
+pub const SPB_SERDE_RAW_BYTES_UNCHECKED: c_int = 2;
 
 // compile-time layout checks (the Rust side of the C header's static_assert in csrc/capi.cu)
 const _: () = assert!(std::mem::size_of::<Fr>() == 32 && std::mem::align_of::<Fr>() <= 16);
@@ -76,6 +79,8 @@ extern "C" {
     // ---- ParamsKZG ----
     pub fn spb_srs_upload(ctx: *mut spb_ctx, k: u32, g: *const G1Affine, g_lagrange: *const G1Affine, out: *mut *mut spb_srs) -> c_int;
     pub fn spb_srs_read_file(ctx: *mut spb_ctx, path: *const c_char, out: *mut *mut spb_srs) -> c_int;
+    /// `format`: SPB_SERDE_RAW_BYTES (checked, upstream's `ParamsKZG::read`) or SPB_SERDE_RAW_BYTES_UNCHECKED
+    pub fn spb_srs_read_file_custom(ctx: *mut spb_ctx, path: *const c_char, format: c_int, out: *mut *mut spb_srs) -> c_int;
     pub fn spb_srs_write_file(ctx: *mut spb_ctx, srs: *const spb_srs, path: *const c_char) -> c_int;
     pub fn spb_srs_download(ctx: *mut spb_ctx, srs: *const spb_srs, basis: c_int, start: usize, count: usize, out: *mut G1Affine) -> c_int;
     pub fn spb_srs_downsize(ctx: *mut spb_ctx, srs: *const spb_srs, k: u32, out: *mut *mut spb_srs) -> c_int;

@@ -47,14 +47,21 @@ impl ParamsKZG<Bn256> {
     }
 }
 
-/// `ParamsKZG::read` for SerdeFormat::RawBytes straight into device memory: the 4 GiB `kzg_bn254_24.srs` never has to be
-/// materialised as `Vec<G1Affine>` when only the prover needs it (b200::spb_srs_read_file). The host vectors are still
-/// needed by the verifier / `write`, so the default `read` path is unchanged; this is the opt-in for prover-only processes.
+/// `ParamsKZG::read` (SerdeFormat::RawBytes, checked) straight into device memory: the 2 GiB `kzg_bn254_24.srs` never has to
+/// be materialised as `Vec<G1Affine>` when only the prover needs it (b200::spb_srs_read_file_custom). As upstream's `read`
+/// does, it rejects a file with a non-canonical coordinate or a point off its curve; the points are checked on the device.
+/// The host vectors are still needed by the verifier / `write`, so the default `read` path is unchanged; this is the opt-in
+/// for prover-only processes.
 pub fn read_params_to_device(path: &std::path::Path) -> Option<(u32, *mut b200::spb_srs)> {
     let ctx = b200::ctx()?;
     let c = std::ffi::CString::new(path.to_str()?).ok()?;
     let mut h = std::ptr::null_mut();
-    if unsafe { b200::spb_srs_read_file(ctx, c.as_ptr(), &mut h) } != 0 {
+    let rc = unsafe { b200::spb_srs_read_file_custom(ctx, c.as_ptr(), b200::SPB_SERDE_RAW_BYTES, &mut h) };
+    if rc == b200::SPB_ERR_DATA {
+        log::warn!("spectre_b200: invalid params file: {}", b200::last_error(ctx));
+        return None;
+    }
+    if rc != 0 {
         log::warn!("spectre_b200: {}", b200::last_error(ctx));
         return None;
     }

@@ -1,4 +1,4 @@
-// BN254 G1 (y^2 = x^3 + 3 over Fq) group law.
+// BN254 G1 (y^2 = x^3 + 3 over Fq) group law, and the validity checks of stored G1 / G2 points.
 //
 // Replaces halo2curves::bn256::{G1, G1Affine} ([UPSTREAM] halo2curves src/bn256/curve.rs + src/derive/curve.rs;
 // types named by the reference at lightclient-circuits/src/util/circuit.rs:12). Conventions kept:
@@ -168,6 +168,44 @@ SPB_HD bool affine_on_curve(const G1Affine& p) {
   Fq lhs = fp_sqr(p.y);
   Fq rhs = fp_add(fp_mul(fp_sqr(p.x), p.x), three);
   return fp_eq(lhs, rhs);
+}
+
+// ---- checks of points read from outside (ParamsKZG::read, SerdeFormat::RawBytes) ----------------------------------------
+// The verdict of a point check. The canonical tests come first: the field arithmetic assumes reduced inputs, so the curve
+// equation is only evaluated on coordinates already known to be less than p.
+enum PointCheck : int { kPointValid = 0, kPointXNotCanonical = 1, kPointYNotCanonical = 2, kPointOffCurve = 3 };
+
+// a G1Affine as stored (raw Montgomery limbs): canonical coordinates and on y^2 = x^3 + 3, or the identity (0, 0)
+SPB_HD int affine_check(const G1Affine& p) {
+  if (!fp_is_canonical(p.x)) return kPointXNotCanonical;
+  if (!fp_is_canonical(p.y)) return kPointYNotCanonical;
+  return affine_on_curve(p) ? kPointValid : kPointOffCurve;
+}
+
+// BN254 G2 affine over Fq2 = Fq[u]/(u^2 + 1): 128 B as stored in a params file (x.c0, x.c1, y.c0, y.c1), identity (0, 0).
+// Only the two points of the params trailer (g2, s_g2) are ever checked, on the host.
+struct alignas(16) Fq2 { Fq c0, c1; };
+struct alignas(16) G2Affine { Fq2 x, y; };
+
+SPB_HD Fq2 fq2_mul(const Fq2& a, const Fq2& b) {
+  Fq2 r;
+  r.c0 = fp_mul_sub_mul(a.c0, b.c0, a.c1, b.c1);  // u^2 = -1
+  r.c1 = fp_add(fp_mul(a.c0, b.c1), fp_mul(a.c1, b.c0));
+  return r;
+}
+
+// canonical coordinates and on the twist y^2 = x^3 + b', b' = 3 / (9 + u), or the identity
+SPB_HD int g2_affine_check(const G2Affine& p) {
+  if (!fp_is_canonical(p.x.c0) || !fp_is_canonical(p.x.c1)) return kPointXNotCanonical;
+  if (!fp_is_canonical(p.y.c0) || !fp_is_canonical(p.y.c1)) return kPointYNotCanonical;
+  if (fp_is_zero(p.x.c0) && fp_is_zero(p.x.c1) && fp_is_zero(p.y.c0) && fp_is_zero(p.y.c1)) return kPointValid;
+  Fq2 b;
+  { constexpr uint32_t v0[8] = SPB_FQ2_TWIST_B_C0_MONT, v1[8] = SPB_FQ2_TWIST_B_C1_MONT; for (int i = 0; i < 8; i++) { b.c0.l[i] = v0[i]; b.c1.l[i] = v1[i]; } }
+  Fq2 lhs = fq2_mul(p.y, p.y);
+  Fq2 rhs = fq2_mul(fq2_mul(p.x, p.x), p.x);
+  rhs.c0 = fp_add(rhs.c0, b.c0);
+  rhs.c1 = fp_add(rhs.c1, b.c1);
+  return fp_eq(lhs.c0, rhs.c0) && fp_eq(lhs.c1, rhs.c1) ? kPointValid : kPointOffCurve;
 }
 
 }  // namespace spb

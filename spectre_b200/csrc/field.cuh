@@ -63,6 +63,17 @@ template <class P> SPB_HD bool fp_eq(const Fp<P>& a, const Fp<P>& b) {
   for (int i = 0; i < 8; i++) t |= a.l[i] ^ b.l[i];
   return t == 0;
 }
+// Are the raw limbs less than the modulus? Every other function here assumes they are, so a value read from outside the
+// library (a params file) is tested with this before any arithmetic touches it. Compared from the top limb down.
+template <class P> SPB_HD bool fp_is_canonical(const Fp<P>& a) {
+  uint32_t lt = 0, eq = 1;
+#pragma unroll
+  for (int i = 7; i >= 0; i--) {
+    lt |= eq & (a.l[i] < P::mod(i) ? 1u : 0u);
+    eq &= a.l[i] == P::mod(i) ? 1u : 0u;
+  }
+  return lt != 0;
+}
 
 #if defined(SPB_LIMB32_PATH)
 // ------------------------------------------------------------------------------------------------

@@ -423,12 +423,74 @@ int spb_srs_downsize(spb_ctx* ctx, const spb_srs* srs, uint32_t k, spb_srs** out
   return 0;
 }
 
-// ParamsKZG::read / write in SerdeFormat::RawBytes: k (u32 LE) | g[n] | g_lagrange[n] | g2 | s_g2, every coordinate as
-// its in-memory Montgomery limbs -- the file halo2-base's gen_srs caches as params/kzg_bn254_{k}.srs
-// ([UPSTREAM] halo2_proofs/src/poly/kzg/commitment.rs; reference .gitignore:36 `params/`). Streamed through two pinned
-// staging buffers straight into device memory, file read and DMA overlapped (K = 24: 4 GiB).
-int spb_srs_read_file(spb_ctx* ctx, const char* path, spb_srs** out) {
+}  // extern "C"
+
+namespace spb {
+
+// Lowest index i < n whose point fails affine_check, folded into *first (all ones before the launch). Only a thread that finds
+// a bad point touches the atomic, and it stops there: its later indices are larger.
+__global__ void __launch_bounds__(256) srs_check_kernel(const G1Affine* pts, uint64_t n, unsigned long long* first) {
+  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x)
+    if (affine_check(pts[i]) != kPointValid) { atomicMin(first, (unsigned long long)i); return; }
+}
+
+static const char* point_check_reason(int verdict) {
+  switch (verdict) {
+    case kPointXNotCanonical: return "x is not less than the field modulus";
+    case kPointYNotCanonical: return "y is not less than the field modulus";
+    case kPointOffCurve: return "not on the curve";
+    default: return "rejected by the device check but valid on the host";
+  }
+}
+
+// Check `count` resident points of device d (one grid-stride launch on d's stream). *bad = index of the first invalid point, or
+// count when every point is valid; *ms accumulates the kernel's device time.
+static int srs_check_points(spb_ctx* ctx, DeviceState& d, const G1Affine* pts, size_t count, size_t* bad, float* ms) {
+  unsigned long long* first = (unsigned long long*)slot(ctx, d, "srs_check", sizeof(unsigned long long));
+  if (!first) return SPB_ERR_OOM;
+  const unsigned tb = 256;
+  const uint64_t blocks = (count + tb - 1) / tb, cap = (uint64_t)(d.sm_count > 0 ? d.sm_count : 1) * 8;
+  SPB_CUDA(ctx, cudaMemsetAsync(first, 0xff, sizeof(unsigned long long), d.stream));
+  SPB_CUDA(ctx, cudaEventRecord(d.ev0, d.stream));
+  srs_check_kernel<<<(unsigned)(blocks < cap ? blocks : cap), tb, 0, d.stream>>>(pts, count, first);
+  SPB_CUDA(ctx, cudaGetLastError());
+  SPB_CUDA(ctx, cudaEventRecord(d.ev1, d.stream));
+  ctx->n_kernel_launches++;
+  unsigned long long h = 0;
+  SPB_CUDA(ctx, cudaMemcpyAsync(&h, first, sizeof h, cudaMemcpyDeviceToHost, d.stream));
+  SPB_CUDA(ctx, cudaStreamSynchronize(d.stream));
+  float t = 0.f;
+  SPB_CUDA(ctx, cudaEventElapsedTime(&t, d.ev0, d.ev1));
+  *ms += t;
+  *bad = h < count ? (size_t)h : count;
+  return 0;
+}
+
+// The shard's first invalid point, downloaded and classified again on the host for the error text.
+static int srs_point_error(spb_ctx* ctx, DeviceState& d, const char* path, const char* basis, const G1Affine* pts, size_t local, size_t global) {
+  G1Affine p;
+  SPB_CUDA(ctx, cudaMemcpyAsync(&p, pts + local, sizeof p, cudaMemcpyDeviceToHost, d.stream));
+  SPB_CUDA(ctx, cudaStreamSynchronize(d.stream));
+  return set_error(ctx, SPB_ERR_DATA, "spb_srs_read_file: %s: %s[%zu]: %s", path, basis, global, point_check_reason(affine_check(p)));
+}
+
+}  // namespace spb
+
+extern "C" {
+
+// ParamsKZG::read_custom / write: k (u32 LE) | g[n] | g_lagrange[n] | g2 | s_g2, every coordinate as its in-memory Montgomery
+// limbs -- the file halo2-base's gen_srs caches as params/kzg_bn254_{k}.srs ([UPSTREAM] halo2_proofs/src/poly/kzg/commitment.rs;
+// reference .gitignore:36 `params/`). Streamed through two pinned staging buffers straight into device memory, file read and
+// DMA overlapped (K = 24: 2 GiB). SPB_SERDE_RAW_BYTES checks every point as halo2curves' read_raw does: the G1 points of each
+// shard with one kernel on its own device once the shard is resident, the G2 trailer on the host. Shards are read in file
+// order, so the first shard that reports a bad point holds the first one of the file. (The check is not fused into the
+// staging loop: on an H100 80GB HBM3 at a 400 W power limit its kernels took 0.9 ms of a 270-300 ms page-cached K = 23 read,
+// tools/srs_read_probe.py.)
+int spb_srs_read_file_custom(spb_ctx* ctx, const char* path, int format, spb_srs** out) {
   if (!ctx || !path || !out) return SPB_ERR_ARG;
+  if (format != SPB_SERDE_RAW_BYTES && format != SPB_SERDE_RAW_BYTES_UNCHECKED)
+    return set_error(ctx, SPB_ERR_ARG, "spb_srs_read_file_custom: unknown format %d (SPB_SERDE_RAW_BYTES or SPB_SERDE_RAW_BYTES_UNCHECKED)", format);
+  const bool checked = format == SPB_SERDE_RAW_BYTES;
   FILE* f = fopen(path, "rb");
   if (!f) return set_error(ctx, SPB_ERR_ARG, "spb_srs_read_file: cannot open %s", path);
   uint32_t k = 0;
@@ -438,6 +500,7 @@ int spb_srs_read_file(spb_ctx* ctx, const char* path, spb_srs** out) {
   {
     std::lock_guard<std::mutex> lk(ctx->mu);
     s = srs_alloc(ctx, k);
+    float check_ms = 0.f;
     for (int which = 0; which < 2 && rc == 0; which++) {
       for (auto& sh : s->shards) {
         DeviceState& d = ctx->dev[sh.dev_index];
@@ -445,16 +508,31 @@ int spb_srs_read_file(spb_ctx* ctx, const char* path, spb_srs** out) {
         G1Affine** dst = which == 0 ? &sh.g : &sh.g_lagrange;
         if (sh.count && cudaMalloc(dst, sh.count * sizeof(G1Affine)) != cudaSuccess) { rc = set_error(ctx, SPB_ERR_OOM, "spb_srs_read_file: cudaMalloc"); break; }
         if (sh.count) rc = stream_file_to_device(ctx, d, f, *dst, sh.count * sizeof(G1Affine), "spb_srs_read_file");
+        if (rc == 0 && checked && sh.count) {
+          size_t bad = sh.count;
+          rc = srs_check_points(ctx, d, *dst, sh.count, &bad, &check_ms);
+          if (rc == 0 && bad < sh.count) rc = srs_point_error(ctx, d, path, which == 0 ? "g" : "g_lagrange", *dst, bad, sh.start + bad);
+        }
         if (rc) break;
       }
     }
     if (rc == 0 && (fread(s->g2, 128, 1, f) != 1 || fread(s->s_g2, 128, 1, f) != 1)) rc = set_error(ctx, SPB_ERR_ARG, "spb_srs_read_file: %s has no G2 trailer", path);
+    for (int i = 0; i < 2 && rc == 0 && checked; i++) {
+      static_assert(sizeof(G2Affine) == 128, "a G2 point of the trailer is 128 bytes");
+      G2Affine q;
+      memcpy(&q, i == 0 ? s->g2 : s->s_g2, sizeof q);
+      const int v = g2_affine_check(q);
+      if (v != kPointValid) rc = set_error(ctx, SPB_ERR_DATA, "spb_srs_read_file: %s: %s: %s", path, i == 0 ? "g2" : "s_g2", point_check_reason(v));
+    }
+    if (rc == 0 && checked) ctx->last_kernel_ms = check_ms;
   }
   fclose(f);
   if (rc) { spb_srs_free(ctx, s); return rc; }
   *out = s;
   return 0;
 }
+
+int spb_srs_read_file(spb_ctx* ctx, const char* path, spb_srs** out) { return spb_srs_read_file_custom(ctx, path, SPB_SERDE_RAW_BYTES_UNCHECKED, out); }
 
 int spb_srs_write_file(spb_ctx* ctx, const spb_srs* srs, const char* path) {
   if (!ctx || !srs || !path) return SPB_ERR_ARG;

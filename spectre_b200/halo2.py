@@ -8,7 +8,7 @@ the reference's own use of them (reference call sites: lightclient-circuits/src/
     halo2_proofs::arithmetic::best_fft            -> best_fft(a, omega, log_n)
     halo2_proofs::arithmetic::best_multiexp       -> best_multiexp(coeffs, bases)
     halo2_proofs::poly::EvaluationDomain          -> EvaluationDomain(j, k)
-    halo2_proofs::poly::kzg::commitment::ParamsKZG-> ParamsKZG.setup / .from_parts / .commit / .commit_lagrange
+    halo2_proofs::poly::kzg::commitment::ParamsKZG-> ParamsKZG.setup / .from_parts / .read_custom / .commit / .commit_lagrange
     arithmetic::{eval_polynomial, kate_division}, ff::BatchInvert -> same names
 
 Field elements are numpy uint64 arrays (..., 4) holding halo2curves' in-memory Montgomery limbs; G1Affine is
@@ -28,6 +28,9 @@ LIB_PATH = os.environ.get("SPB_LIB_PATH") or os.path.join(_HERE, "libspectre_b20
 
 BASIS_G = 0
 BASIS_G_LAGRANGE = 1
+
+ERR_DATA = -6                                                     # SPB_ERR_DATA: invalid input data
+SERDE_FORMATS = {"RawBytes": 1, "RawBytesUnchecked": 2}          # SPB_SERDE_RAW_BYTES, SPB_SERDE_RAW_BYTES_UNCHECKED
 
 
 class BackendError(RuntimeError):
@@ -488,9 +491,26 @@ class ParamsKZG:
 
     @classmethod
     def read(cls, backend, path):
-        """ParamsKZG::read(reader) for SerdeFormat::RawBytes (the params/kzg_bn254_{k}.srs cache of gen_srs)."""
+        """Read a params file in the RawBytes layout (the params/kzg_bn254_{k}.srs cache of gen_srs) WITHOUT validating the
+        points (spb_srs_read_file). Upstream's ParamsKZG::read checks them: that is read_custom(backend, path, "RawBytes")."""
         h = ctypes.c_void_p()
         backend.check(backend.lib.spb_srs_read_file(backend.ctx, path.encode(), ctypes.byref(h)), "spb_srs_read_file")
+        return cls._from_read(backend, h)
+
+    @classmethod
+    def read_custom(cls, backend, path, format):
+        """ParamsKZG::read_custom(reader, format). format "RawBytes": every coordinate must be canonical and every point on its
+        curve, else BackendError naming the first invalid point (SPB_ERR_DATA, halo2's io::ErrorKind::InvalidData);
+        "RawBytesUnchecked": no checks."""
+        if format not in SERDE_FORMATS:
+            raise ValueError("read_custom: format must be one of %s (the compressed Processed format is not implemented)" % sorted(SERDE_FORMATS))
+        h = ctypes.c_void_p()
+        backend.check(backend.lib.spb_srs_read_file_custom(backend.ctx, path.encode(), ctypes.c_int(SERDE_FORMATS[format]), ctypes.byref(h)),
+                      "spb_srs_read_file_custom")
+        return cls._from_read(backend, h)
+
+    @classmethod
+    def _from_read(cls, backend, h):
         backend.lib.spb_srs_k.restype = ctypes.c_uint32
         backend.lib.spb_srs_k.argtypes = [ctypes.c_void_p]
         return cls(backend, int(backend.lib.spb_srs_k(h)), h)
