@@ -92,23 +92,24 @@ def test_product_library_has_no_cpu_stand_in(libpath):
     assert " orc_" not in syms
 
 
-def _build_cpp_mirror(libpath):
-    exe = os.path.join(ROOT, "tests", "cpp", "host_mirror")
-    src = exe + ".cpp"
+def _build_cpp_mirror(libpath, out_dir):
+    """the executable goes to out_dir: the checkout may be read-only"""
+    exe = os.path.join(str(out_dir), "host_mirror")
+    src = os.path.join(ROOT, "tests", "cpp", "host_mirror.cpp")
     libdir = os.path.dirname(libpath)
     subprocess.check_call(["g++", "-std=c++17", "-O1", "-o", exe, src, "-L" + libdir, "-lspectre_b200", "-Wl,-rpath," + libdir])
     return exe
 
 
-def test_cpp_host_mirror_compiles_and_links(libpath):
+def test_cpp_host_mirror_compiles_and_links(libpath, tmp_path):
     """include/spectre_b200.hpp (the compiled-language host side) builds against the C ABI."""
-    exe = _build_cpp_mirror(libpath)
+    exe = _build_cpp_mirror(libpath, tmp_path)
     assert subprocess.check_output([exe], text=True).strip() == "linked"
 
 
 @pytest.mark.gpu
-def test_cpp_host_mirror_runs(libpath):
-    exe = _build_cpp_mirror(libpath)
+def test_cpp_host_mirror_runs(libpath, tmp_path):
+    exe = _build_cpp_mirror(libpath, tmp_path)
     out = subprocess.run([exe, "run"], capture_output=True, text=True)
     assert out.returncode == 0 and "host mirror ok" in out.stdout, out.stdout + out.stderr
 

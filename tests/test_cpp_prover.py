@@ -205,14 +205,14 @@ def test_cpp_driver_reproduces_the_python_proof(orc, tmp_path, shape, k, chacha_
         assert f.read() == proof
 
 
-def _build_main_against_the_real_library():
+def _build_main_against_the_real_library(out_dir):
     from tools import cpp_driver
-    return cpp_driver.build_main_against_the_real_library()
+    return cpp_driver.build_main_against_the_real_library(str(out_dir))
 
 
-def test_cpp_driver_links_against_the_real_library():
+def test_cpp_driver_links_against_the_real_library(tmp_path):
     """the same main builds with CudaMemory against libspectre_b200.so + cudart (every ABI symbol the driver uses exists there)"""
-    assert os.path.exists(_build_main_against_the_real_library())
+    assert os.path.exists(_build_main_against_the_real_library(tmp_path))
 
 
 def _dump_case(*args):
@@ -226,7 +226,7 @@ def test_cpp_driver_on_the_gpu_reproduces_the_oracle_proof(orc, tmp_path):
     the same proof bytes as the Python driver on the CPU oracle, proved twice in the same process."""
     from spectre_b200 import circuits, plonk
     from tests.plonk_oracle_engine import OracleEngine, SeededRng
-    exe = _build_main_against_the_real_library()
+    exe = _build_main_against_the_real_library(tmp_path)
     k, instances = 8, [7, 8, 9]
     cs = circuits.halo2lib_shape(3, 2)
     fixed, adv, copies = circuits.halo2lib_witness(cs, k, instances, lookup_bits=4, groups=20, num_gate_advice=3, num_lookup_advice=2)
@@ -251,7 +251,7 @@ def test_cpp_driver_on_the_gpu_reproduces_the_contract_accepted_k23_fixture(orc,
     import json
     from spectre_b200 import circuits
     from tests.plonk_oracle_engine import SeededRng
-    exe = _build_main_against_the_real_library()
+    exe = _build_main_against_the_real_library(tmp_path)
     with open(os.path.join(ROOT, "tests", "golden", "aggregation_k23_proof.json")) as f:
         fx = json.load(f)
     k, n = fx["k"], 1 << fx["k"]

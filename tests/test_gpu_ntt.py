@@ -12,7 +12,7 @@ def _omega(orc, k):
     return orc.fr([pyref.omega(k)])[0]
 
 
-@pytest.mark.parametrize("k", [0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15, 16, 17, 19, 20])
+@pytest.mark.parametrize("k", [0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15, 16, 17, 18, 19, 20])
 def test_best_fft_matches_oracle(be, orc, k):
     a = orc.fr_random_chacha(1 << k, 0x5eed0001 + k)
     w = _omega(orc, k)

@@ -3,6 +3,7 @@ against libspectre_b200.so: build the binary, dump a circuit instance in the for
 Used by tests/test_cpp_prover.py (parity) and bench.py (timing next to the Python driver). No oracle involved."""
 import os
 import subprocess
+import tempfile
 
 import numpy as np
 
@@ -11,11 +12,11 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 def build_main_against_the_real_library(out_dir=None):
     """g++ tests/cpp/prover_main.cpp -DSPB_PROVER_WITH_CUDART against libspectre_b200.so + cudart -> <out_dir>/prover_main_cuda
-    (default out_dir: tests/cpp)"""
+    (default out_dir: a new temporary directory -- the checkout may be read-only)"""
     from spectre_b200 import build
     lib = build.build()
     libdir = os.path.dirname(lib)
-    exe = os.path.join(out_dir or os.path.join(ROOT, "tests", "cpp"), "prover_main_cuda")
+    exe = os.path.join(out_dir or tempfile.mkdtemp(prefix="spb_prover_main_"), "prover_main_cuda")
     src = os.path.join(ROOT, "tests", "cpp", "prover_main.cpp")
     hdrs = [os.path.join(ROOT, "include", h) for h in ("spectre_b200.h", "spectre_b200_prover.hpp")]
     if os.path.exists(exe) and os.path.getmtime(exe) >= max(os.path.getmtime(p) for p in [src, lib] + hdrs):
