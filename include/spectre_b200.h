@@ -201,6 +201,9 @@ int spb_lagrange_to_coeff_batch_dev(spb_ctx* ctx, const spb_domain* d, spb_fr* c
 int spb_coeff_to_extended_batch_dev(spb_ctx* ctx, const spb_domain* d, const spb_fr* const* d_in, spb_fr* const* d_out, size_t count);
 
 /* ---- batch polynomial arithmetic ([UPSTREAM] halo2_proofs/src/arithmetic.rs, ff::BatchInvert) ---------- */
+/* Zero-length inputs: with n = 0, spb_vec_{mul,axpy,scale}, spb_grand_product, spb_batch_invert (host and _dev forms),
+ * spb_grand_product_seeded_dev, spb_fr_random_chacha_dev, spb_lincomb_dev, spb_weighted_sum_dev and spb_g1_fixed_base_mul
+ * return 0 without touching the device; spb_eval_polynomial(_dev) returns 0 with *out = 0. */
 /* a[i] <- a[i]^-1, zeros stay zero (BatchInvert semantics) */
 int spb_batch_invert(spb_ctx* ctx, spb_fr* a, size_t n);
 /* eval_polynomial(poly, point) */

@@ -29,7 +29,10 @@ void* slot(spb_ctx* ctx, DeviceState& d, const char* name, size_t bytes) {
   if (b.ptr) { cudaStreamSynchronize(d.stream); cudaFree(b.ptr); b.ptr = nullptr; b.cap = 0; }
   size_t want = bytes + bytes / 8;  // a little headroom so growing sizes do not realloc every call
   cudaError_t e = cudaMalloc(&b.ptr, want);
-  if (e != cudaSuccess) { want = bytes; e = cudaMalloc(&b.ptr, want); }
+  if (e != cudaSuccess) {
+    cudaGetLastError();  // the failed headroom allocation must not be reported by the next launch check
+    want = bytes; e = cudaMalloc(&b.ptr, want);
+  }
   if (e != cudaSuccess) { set_error(ctx, SPB_ERR_OOM, "cudaMalloc(%zu) for slot %s: %s", want, name, cudaGetErrorString(e)); b.ptr = nullptr; return nullptr; }
   b.cap = want;
   return b.ptr;
@@ -187,7 +190,7 @@ spb_ctx* spb_init(const int* device_ids, int n_dev) {
       cudaSetDevice(ctx->dev[i].device);
       cudaError_t e = cudaDeviceEnablePeerAccess(ctx->dev[j].device, 0);
       if (e != cudaSuccess && e != cudaErrorPeerAccessAlreadyEnabled) ctx->peer_access = false;
-      cudaGetLastError();
+      cudaGetLastError();  // a peer-access failure is tolerated and must not be reported by the next launch check
     }
   if (!ctx->dev.empty()) cudaSetDevice(ctx->dev[0].device);
   return ctx;
@@ -238,9 +241,7 @@ void* spb_stream(spb_ctx* ctx, int dev_index) {
 // ---- file <-> device (params / proving-key files: SURVEY.md 8f rank 4) -----------------------------------------------------
 int spb_read_file_dev(spb_ctx* ctx, const char* path, uint64_t offset, void* d_dst, size_t bytes) {
   if (!ctx || !path || (bytes && !d_dst)) return SPB_ERR_ARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  DeviceState& d = ctx->dev[0];
-  SPB_CUDA(ctx, cudaSetDevice(d.device));
+  SPB_ENTER(ctx);
   FILE* f = fopen(path, "rb");
   if (!f) return set_error(ctx, SPB_ERR_ARG, "spb_read_file_dev: cannot open %s", path);
   int rc = fseeko(f, (off_t)offset, SEEK_SET) == 0 ? stream_file_to_device(ctx, d, f, d_dst, bytes, "spb_read_file_dev") : set_error(ctx, SPB_ERR_ARG, "spb_read_file_dev: seek failed");
@@ -249,9 +250,7 @@ int spb_read_file_dev(spb_ctx* ctx, const char* path, uint64_t offset, void* d_d
 }
 int spb_write_file_dev(spb_ctx* ctx, const char* path, int append, const void* d_src, size_t bytes) {
   if (!ctx || !path || (bytes && !d_src)) return SPB_ERR_ARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  DeviceState& d = ctx->dev[0];
-  SPB_CUDA(ctx, cudaSetDevice(d.device));
+  SPB_ENTER(ctx);
   FILE* f = fopen(path, append ? "ab" : "wb");
   if (!f) return set_error(ctx, SPB_ERR_ARG, "spb_write_file_dev: cannot open %s", path);
   int rc = stream_device_to_file(ctx, d, f, d_src, bytes, "spb_write_file_dev");
@@ -302,11 +301,8 @@ static int ntt_timed(spb_ctx* ctx, DeviceState& d, const Fr* src, Fr* dst, uint3
 
 int spb_ntt_dev(spb_ctx* ctx, spb_fr* d_a, uint32_t log_n, const spb_fr* omega) {
   if (!ctx || !d_a || !omega) return SPB_ERR_ARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  DeviceState& d = ctx->dev[0];
-  SPB_CUDA(ctx, cudaSetDevice(d.device));
-  Fr w; memcpy(&w, omega, 32);
-  return ntt_timed(ctx, d, (const Fr*)d_a, (Fr*)d_a, log_n, w, NttOpts());
+  SPB_ENTER(ctx);
+  return ntt_timed(ctx, d, (const Fr*)d_a, (Fr*)d_a, log_n, fr_load(omega), NttOpts());
 }
 
 // host-buffer transform through a device staging slot
@@ -319,23 +315,16 @@ static int ntt_host(spb_ctx* ctx, const Fr* in, size_t n_in_copy, Fr* out, size_
   }
   DeviceState& d = ctx->dev[0];
   SPB_CUDA(ctx, cudaSetDevice(d.device));
-  size_t n = (size_t)1 << k;
-  Fr* buf = (Fr*)slot(ctx, d, "ntt_io", n * sizeof(Fr));
-  if (!buf) return SPB_ERR_OOM;
-  SPB_CUDA(ctx, cudaMemcpyAsync(buf, in, n_in_copy * sizeof(Fr), cudaMemcpyHostToDevice, d.stream));
-  SPB_TRY(ntt_timed(ctx, d, buf, buf, k, omega, o));
-  SPB_CUDA(ctx, cudaMemcpyAsync(out, buf, n_out_copy * sizeof(Fr), cudaMemcpyDeviceToHost, d.stream));
-  SPB_CUDA(ctx, cudaStreamSynchronize(d.stream));
-  return 0;
+  return run_staged(ctx, d, {{"ntt_io", ((size_t)1 << k) * sizeof(Fr), in, out, n_in_copy * sizeof(Fr), n_out_copy * sizeof(Fr)}},
+                    [&](void* const* p) { return ntt_timed(ctx, d, (Fr*)p[0], (Fr*)p[0], k, omega, o); });
 }
 
 int spb_ntt(spb_ctx* ctx, spb_fr* a, uint32_t log_n, const spb_fr* omega) {
   if (!ctx || !a || !omega) return SPB_ERR_ARG;
   if (log_n > 28) return set_error(ctx, SPB_ERR_ARG, "spb_ntt: log_n %u > 28", log_n);
   std::lock_guard<std::mutex> lk(ctx->mu);
-  Fr w; memcpy(&w, omega, 32);
   size_t n = (size_t)1 << log_n;
-  return ntt_host(ctx, (const Fr*)a, n, (Fr*)a, n, log_n, w, NttOpts());
+  return ntt_host(ctx, (const Fr*)a, n, (Fr*)a, n, log_n, fr_load(omega), NttOpts());
 }
 
 // ---- EvaluationDomain --------------------------------------------------------------------------------------
@@ -362,12 +351,9 @@ int spb_domain_new(spb_ctx* ctx, uint32_t j, uint32_t k, spb_domain** out) {
   while ((1ull << ek) < n * dm->quotient_poly_degree) ek++;
   if (ek > 28) { delete dm; return set_error(ctx, SPB_ERR_ARG, "domain: extended_k %u > 28", ek); }
   dm->extended_k = ek;
-  Fr w; { constexpr uint32_t v[8] = SPB_FR_ROOT_OF_UNITY_MONT; for (int i = 0; i < 8; i++) w.l[i] = v[i]; }
-  for (uint32_t i = ek; i < 28; i++) w = fp_sqr(w);
-  dm->extended_omega = w; dm->extended_omega_inv = fp_inv(w);
-  for (uint32_t i = k; i < ek; i++) w = fp_sqr(w);
-  dm->omega = w; dm->omega_inv = fp_inv(w);
-  { constexpr uint32_t v[8] = SPB_FR_ZETA_MONT; for (int i = 0; i < 8; i++) dm->g_coset.l[i] = v[i]; }
+  dm->extended_omega = fr_root_of_unity(ek); dm->extended_omega_inv = fp_inv(dm->extended_omega);
+  dm->omega = fr_root_of_unity(k); dm->omega_inv = fp_inv(dm->omega);
+  dm->g_coset = fr_zeta();
   dm->g_coset_inv = fp_sqr(dm->g_coset);
   dm->ifft_divisor = fp_inv(fr_from_u64(n));
   dm->extended_ifft_divisor = fp_inv(fr_from_u64(1ull << ek));
@@ -377,9 +363,7 @@ int spb_domain_new(spb_ctx* ctx, uint32_t j, uint32_t k, spb_domain** out) {
   SPB_CUDA(ctx, cudaSetDevice(d.device));
   SPB_CUDA(ctx, cudaMalloc(&dm->d_t_evaluations, dm->t_len * sizeof(Fr)));
   Fr cur0 = fp_pow_u64(dm->g_coset, n), step = fp_pow_u64(dm->extended_omega, n);
-  vanishing_table_kernel<<<(dm->t_len + 63) / 64, 64, 0, d.stream>>>(dm->d_t_evaluations, cur0, step, dm->t_len);
-  SPB_CUDA(ctx, cudaGetLastError());
-  ctx->n_kernel_launches++;
+  SPB_TRY(launch(ctx, d.stream, nblk(dm->t_len, 64), 64, 0, vanishing_table_kernel, dm->d_t_evaluations, cur0, step, dm->t_len));
   SPB_CUDA(ctx, cudaStreamSynchronize(d.stream));
   *out = dm;
   return 0;
@@ -436,43 +420,29 @@ int spb_extended_to_coeff(spb_ctx* ctx, const spb_domain* dm, const spb_fr* in, 
 }
 static int div_vanishing_device(spb_ctx* ctx, DeviceState& d, const spb_domain* dm, Fr* d_a) {
   uint64_t e = 1ull << dm->extended_k;
-  mul_periodic_kernel<<<(unsigned)((e + 255) / 256), 256, 0, d.stream>>>(d_a, dm->d_t_evaluations, e, dm->t_len - 1);
-  SPB_CUDA(ctx, cudaGetLastError());
-  ctx->n_kernel_launches++;
-  return 0;
+  return launch(ctx, d.stream, nblk(e, 256), 256, 0, mul_periodic_kernel, d_a, dm->d_t_evaluations, e, dm->t_len - 1);
 }
 int spb_divide_by_vanishing(spb_ctx* ctx, const spb_domain* dm, spb_fr* a) {
   if (!ctx || !dm || !a) return SPB_ERR_ARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  DeviceState& d = ctx->dev[0];
-  SPB_CUDA(ctx, cudaSetDevice(d.device));
-  size_t e = (size_t)1 << dm->extended_k;
-  Fr* buf = (Fr*)slot(ctx, d, "ntt_io", e * sizeof(Fr));
-  if (!buf) return SPB_ERR_OOM;
-  SPB_CUDA(ctx, cudaMemcpyAsync(buf, a, e * sizeof(Fr), cudaMemcpyHostToDevice, d.stream));
-  SPB_TRY(div_vanishing_device(ctx, d, dm, buf));
-  SPB_CUDA(ctx, cudaMemcpyAsync(a, buf, e * sizeof(Fr), cudaMemcpyDeviceToHost, d.stream));
-  SPB_CUDA(ctx, cudaStreamSynchronize(d.stream));
-  return 0;
+  SPB_ENTER(ctx);
+  return run_staged(ctx, d, {{"ntt_io", ((size_t)1 << dm->extended_k) * sizeof(Fr), a, a}},
+                    [&](void* const* p) { return div_vanishing_device(ctx, d, dm, (Fr*)p[0]); });
 }
 int spb_lagrange_to_coeff_dev(spb_ctx* ctx, const spb_domain* dm, spb_fr* d_a) {
   if (!ctx || !dm || !d_a) return SPB_ERR_ARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  DeviceState& d = ctx->dev[0]; SPB_CUDA(ctx, cudaSetDevice(d.device));
+  SPB_ENTER(ctx);
   Fr post[3]; NttOpts o; l2c_opts(dm, post, o);
   return ntt_timed(ctx, d, (const Fr*)d_a, (Fr*)d_a, dm->k, dm->omega_inv, o);
 }
 int spb_coeff_to_extended_dev(spb_ctx* ctx, const spb_domain* dm, const spb_fr* d_in, spb_fr* d_out) {
   if (!ctx || !dm || !d_in || !d_out) return SPB_ERR_ARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  DeviceState& d = ctx->dev[0]; SPB_CUDA(ctx, cudaSetDevice(d.device));
+  SPB_ENTER(ctx);
   Fr pre[3]; NttOpts o; c2e_opts(dm, pre, o);
   return ntt_timed(ctx, d, (const Fr*)d_in, (Fr*)d_out, dm->extended_k, dm->extended_omega, o);
 }
 int spb_extended_to_coeff_dev(spb_ctx* ctx, const spb_domain* dm, const spb_fr* d_in, spb_fr* d_out) {
   if (!ctx || !dm || !d_in || !d_out) return SPB_ERR_ARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  DeviceState& d = ctx->dev[0]; SPB_CUDA(ctx, cudaSetDevice(d.device));
+  SPB_ENTER(ctx);
   Fr post[3]; NttOpts o; e2c_opts(dm, post, o);
   return ntt_timed(ctx, d, (const Fr*)d_in, (Fr*)d_out, dm->extended_k, dm->extended_omega_inv, o);
 }
@@ -518,8 +488,7 @@ int spb_coeff_to_extended_batch_dev(spb_ctx* ctx, const spb_domain* dm, const sp
 }
 int spb_divide_by_vanishing_dev(spb_ctx* ctx, const spb_domain* dm, spb_fr* d_a) {
   if (!ctx || !dm || !d_a) return SPB_ERR_ARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  DeviceState& d = ctx->dev[0]; SPB_CUDA(ctx, cudaSetDevice(d.device));
+  SPB_ENTER(ctx);
   SPB_TRY(div_vanishing_device(ctx, d, dm, (Fr*)d_a));
   SPB_CUDA(ctx, cudaStreamSynchronize(d.stream));
   return 0;
@@ -528,18 +497,13 @@ int spb_divide_by_vanishing_dev(spb_ctx* ctx, const spb_domain* dm, spb_fr* d_a)
 // ---- test utilities ----------------------------------------------------------------------------------------
 int spb_test_field_op(spb_ctx* ctx, int field, int op, const spb_fr* a, const spb_fr* b, spb_fr* out, size_t n) {
   if (!ctx || !a || !b || !out) return SPB_ERR_ARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  DeviceState& d = ctx->dev[0];
-  SPB_CUDA(ctx, cudaSetDevice(d.device));
+  SPB_ENTER(ctx);
   Fr* buf = (Fr*)slot(ctx, d, "test_io", 3 * n * sizeof(Fr));
   if (!buf) return SPB_ERR_OOM;
   SPB_CUDA(ctx, cudaMemcpyAsync(buf, a, n * 32, cudaMemcpyHostToDevice, d.stream));
   SPB_CUDA(ctx, cudaMemcpyAsync(buf + n, b, n * 32, cudaMemcpyHostToDevice, d.stream));
-  unsigned blocks = (unsigned)((n + 127) / 128);
-  if (field == 0) field_op_kernel<FrParams><<<blocks, 128, 0, d.stream>>>(op, (const Fr*)buf, (const Fr*)(buf + n), (Fr*)(buf + 2 * n), n);
-  else field_op_kernel<FqParams><<<blocks, 128, 0, d.stream>>>(op, (const Fq*)buf, (const Fq*)(buf + n), (Fq*)(buf + 2 * n), n);
-  SPB_CUDA(ctx, cudaGetLastError());
-  ctx->n_kernel_launches++;
+  if (field == 0) SPB_TRY(launch(ctx, d.stream, nblk(n, 128), 128, 0, field_op_kernel<FrParams>, op, (const Fr*)buf, (const Fr*)(buf + n), (Fr*)(buf + 2 * n), n));
+  else SPB_TRY(launch(ctx, d.stream, nblk(n, 128), 128, 0, field_op_kernel<FqParams>, op, (const Fq*)buf, (const Fq*)(buf + n), (Fq*)(buf + 2 * n), n));
   SPB_CUDA(ctx, cudaMemcpyAsync(out, buf + 2 * n, n * 32, cudaMemcpyDeviceToHost, d.stream));
   SPB_CUDA(ctx, cudaStreamSynchronize(d.stream));
   return 0;
@@ -547,28 +511,17 @@ int spb_test_field_op(spb_ctx* ctx, int field, int op, const spb_fr* a, const sp
 
 int spb_bench_modmul(spb_ctx* ctx, int field, uint32_t threads, uint32_t iters, int ilp, float* ms) {
   if (!ctx || !ms) return SPB_ERR_ARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  DeviceState& d = ctx->dev[0];
-  SPB_CUDA(ctx, cudaSetDevice(d.device));
+  SPB_ENTER(ctx);
   threads = (threads + 255) / 256 * 256;
   Fr* buf = (Fr*)slot(ctx, d, "test_io", (size_t)threads * sizeof(Fr));
   if (!buf) return SPB_ERR_OOM;
   SPB_CUDA(ctx, cudaEventRecord(d.ev0, d.stream));
-  unsigned blocks = threads / 256;
-  if (ilp & 0x100) {  // squaring chains (two independent ones per thread)
-    if (field == 0) modmul_bench_kernel<FrParams, 2, true><<<blocks, 256, 0, d.stream>>>((Fr*)buf, iters);
-    else modmul_bench_kernel<FqParams, 2, true><<<blocks, 256, 0, d.stream>>>((Fq*)buf, iters);
-  } else if (field == 0) {
-    if (ilp == 1) modmul_bench_kernel<FrParams, 1><<<blocks, 256, 0, d.stream>>>((Fr*)buf, iters);
-    else if (ilp == 2) modmul_bench_kernel<FrParams, 2><<<blocks, 256, 0, d.stream>>>((Fr*)buf, iters);
-    else modmul_bench_kernel<FrParams, 4><<<blocks, 256, 0, d.stream>>>((Fr*)buf, iters);
-  } else {
-    if (ilp == 1) modmul_bench_kernel<FqParams, 1><<<blocks, 256, 0, d.stream>>>((Fq*)buf, iters);
-    else if (ilp == 2) modmul_bench_kernel<FqParams, 2><<<blocks, 256, 0, d.stream>>>((Fq*)buf, iters);
-    else modmul_bench_kernel<FqParams, 4><<<blocks, 256, 0, d.stream>>>((Fq*)buf, iters);
-  }
-  SPB_CUDA(ctx, cudaGetLastError());
-  ctx->n_kernel_launches++;
+  // ilp & 0x100: squaring chains (two independent ones per thread)
+  void (*fr)(Fr*, uint32_t) = (ilp & 0x100) ? modmul_bench_kernel<FrParams, 2, true> : ilp == 1 ? modmul_bench_kernel<FrParams, 1>
+                              : ilp == 2 ? modmul_bench_kernel<FrParams, 2> : modmul_bench_kernel<FrParams, 4>;
+  void (*fq)(Fq*, uint32_t) = (ilp & 0x100) ? modmul_bench_kernel<FqParams, 2, true> : ilp == 1 ? modmul_bench_kernel<FqParams, 1>
+                              : ilp == 2 ? modmul_bench_kernel<FqParams, 2> : modmul_bench_kernel<FqParams, 4>;
+  SPB_TRY(field == 0 ? launch(ctx, d.stream, threads / 256, 256, 0, fr, (Fr*)buf, iters) : launch(ctx, d.stream, threads / 256, 256, 0, fq, (Fq*)buf, iters));
   SPB_CUDA(ctx, cudaEventRecord(d.ev1, d.stream));
   SPB_CUDA(ctx, cudaStreamSynchronize(d.stream));
   SPB_CUDA(ctx, cudaEventElapsedTime(ms, d.ev0, d.ev1));

@@ -3,6 +3,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
+#include <string.h>
+#include <initializer_list>
 #include <map>
 #include <mutex>
 #include <string>
@@ -88,6 +90,62 @@ void* slot(spb_ctx* ctx, DeviceState& d, const char* name, size_t bytes);
     if (rc_ != 0) return rc_;    \
   } while (0)
 
+// Prologue of an entry point that works on the first device of the context: takes the context lock, binds `d`.
+#define SPB_ENTER(ctx)                          \
+  std::lock_guard<std::mutex> lk((ctx)->mu);    \
+  DeviceState& d = (ctx)->dev[0];               \
+  SPB_CUDA(ctx, cudaSetDevice(d.device));
+
+inline unsigned nblk(uint64_t n, unsigned t) { return (unsigned)((n + t - 1) / t); }
+
+// Every kernel of the library is launched through here. An empty grid launches nothing and returns 0. Otherwise the launch is
+// checked, so no launch error is left pending for a later, unrelated call, and counted: the context's launch counter
+// (spb_kernel_launches) counts the library's own __global__ launches, not CUB's internal ones, memsets or copies.
+template <class... P, class... A>
+int launch(spb_ctx* ctx, cudaStream_t stream, dim3 grid, dim3 block, size_t smem, void (*kernel)(P...), const A&... args) {
+  if (!grid.x || !grid.y || !grid.z) return 0;
+  kernel<<<grid, block, smem, stream>>>(args...);
+  ctx->n_kernel_launches++;
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess)
+    return set_error(ctx, SPB_ERR_CUDA, "kernel launch (grid %ux%ux%u, block %u, %zu B shared memory): %s", grid.x, grid.y, grid.z,
+                     block.x * block.y * block.z, smem, cudaGetErrorString(e));
+  return 0;
+}
+
+// One device buffer of a host-buffer entry point: slot `slot` of `bytes` bytes. Before the device core runs, its first
+// `in_bytes` are copied from `in`; after it, its first `out_bytes` are copied to `out` (a null pointer: no copy).
+struct Staging {
+  const char* slot;
+  size_t bytes;
+  const void* in;
+  void* out;
+  size_t in_bytes = bytes, out_bytes = bytes;
+};
+// The host-buffer form of a device core: stages every buffer in its slot, uploads, runs core(device pointers, in the order of
+// `bufs`) on d.stream, downloads and synchronises.
+template <class Core>
+int run_staged(spb_ctx* ctx, DeviceState& d, std::initializer_list<Staging> bufs, Core&& core) {
+  std::vector<void*> p;
+  for (const Staging& b : bufs) {
+    p.push_back(slot(ctx, d, b.slot, b.bytes));
+    if (!p.back()) return SPB_ERR_OOM;
+  }
+  size_t i = 0;
+  for (const Staging& b : bufs) {
+    if (b.in) SPB_CUDA(ctx, cudaMemcpyAsync(p[i], b.in, b.in_bytes, cudaMemcpyHostToDevice, d.stream));
+    i++;
+  }
+  SPB_TRY(core(p.data()));
+  i = 0;
+  for (const Staging& b : bufs) {
+    if (b.out) SPB_CUDA(ctx, cudaMemcpyAsync(b.out, p[i], b.out_bytes, cudaMemcpyDeviceToHost, d.stream));
+    i++;
+  }
+  SPB_CUDA(ctx, cudaStreamSynchronize(d.stream));
+  return 0;
+}
+
 // ---- capi.cu: multi-device sharding of one pass ----
 // Row ranges of a pass over `rows` rows, one per device, starting at multiples of 256 rows; a single range on the first device
 // when the context has one device, no peer access, or the pass is short enough to be launch-bound.
@@ -125,5 +183,16 @@ inline Fr fr_from_u64(uint64_t v) {
   Fr a = fp_zero<FrParams>(); a.l[0] = (uint32_t)v; a.l[1] = (uint32_t)(v >> 32);
   return fp_to_mont(a);
 }
+inline Fr fr_load(const spb_fr* p) { Fr a; memcpy(&a, p, 32); return a; }
+inline Fr fr_const(const uint32_t (&v)[8]) { Fr a; for (int i = 0; i < 8; i++) a.l[i] = v[i]; return a; }
+// primitive 2^k-th root of unity (Montgomery form)
+inline Fr fr_root_of_unity(uint32_t k) {
+  constexpr uint32_t v[8] = SPB_FR_ROOT_OF_UNITY_MONT;
+  Fr w = fr_const(v);
+  for (uint32_t i = k; i < SPB_FR_S; i++) w = fp_sqr(w);
+  return w;
+}
+inline Fr fr_zeta() { constexpr uint32_t v[8] = SPB_FR_ZETA_MONT; return fr_const(v); }
+inline Fr fr_delta() { constexpr uint32_t v[8] = SPB_FR_DELTA_MONT; return fr_const(v); }
 
 }  // namespace spb

@@ -92,21 +92,18 @@ int radix_sort_pairs_u64(spb_ctx* ctx, DeviceState& d, unsigned long long* keys_
   const uint32_t ntiles = (uint32_t)((n + kRsTile - 1) / kRsTile);
   SPB_CUDA(ctx, cudaMemsetAsync(hist, 0, 8 * 256 * 4, d.stream));
   unsigned hb = ntiles < (unsigned)d.sm_count * 4 ? ntiles : (unsigned)d.sm_count * 4;
-  rs_hist_all_kernel<<<hb ? hb : 1, kRsThreads, 0, d.stream>>>(keys_a, n, hist);
+  SPB_TRY(launch(ctx, d.stream, hb ? hb : 1, kRsThreads, 0, rs_hist_all_kernel, keys_a, n, hist));
   uint32_t h[8 * 256];
   SPB_CUDA(ctx, cudaMemcpyAsync(h, hist, sizeof h, cudaMemcpyDeviceToHost, d.stream));
   SPB_CUDA(ctx, cudaStreamSynchronize(d.stream));
-  ctx->n_kernel_launches++;
   int passes = 0;
   for (int dg = 0; dg < 8; dg++) {
     bool trivial = false;
     for (int b = 0; b < 256; b++) if (h[dg * 256 + b] == n) trivial = true;
     if (trivial) continue;
-    rs_tile_hist_kernel<<<ntiles, kRsThreads, 0, d.stream>>>(keys_a, n, 8 * dg, ntiles, tile_hist);
+    SPB_TRY(launch(ctx, d.stream, ntiles, kRsThreads, 0, rs_tile_hist_kernel, keys_a, n, 8 * dg, ntiles, tile_hist));
     SPB_CUDA(ctx, cub::DeviceScan::ExclusiveSum(scan_tmp, scan_bytes, tile_hist, tile_hist, (int)(256 * ntiles), d.stream));
-    rs_scatter_kernel<<<ntiles, kRsThreads, 0, d.stream>>>(keys_a, idx_a, keys_b, idx_b, n, 8 * dg, ntiles, tile_hist);
-    SPB_CUDA(ctx, cudaGetLastError());
-    ctx->n_kernel_launches += 2;
+    SPB_TRY(launch(ctx, d.stream, ntiles, kRsThreads, 0, rs_scatter_kernel, keys_a, idx_a, keys_b, idx_b, n, 8 * dg, ntiles, tile_hist));
     unsigned long long* tk = keys_a; keys_a = keys_b; keys_b = tk;
     uint32_t* ti = idx_a; idx_a = idx_b; idx_b = ti;
     passes++;
@@ -175,19 +172,15 @@ __global__ void lk_emit_leftover_kernel(const Fr* stb, const uint32_t* left_flag
 }
 
 namespace {
-inline unsigned nb(uint64_t n) { return (unsigned)((n + 255) / 256); }
-
 // sorted[i] = canonical values of src in ascending order (idx/keys/scratch are n-sized work arrays)
 int sort_canonical(spb_ctx* ctx, DeviceState& d, const Fr* src, Fr* canon, Fr* sorted, uint32_t* idx_a, uint32_t* idx_b, unsigned long long* keys_a,
                    unsigned long long* keys_b, uint32_t* hist, uint32_t* tile_hist, void* tmp, size_t tmp_bytes, uint64_t n) {
-  lk_canon_kernel<<<nb(n), 256, 0, d.stream>>>(src, canon, idx_a, n);
+  SPB_TRY(launch(ctx, d.stream, nblk(n, 256), 256, 0, lk_canon_kernel, src, canon, idx_a, n));
   for (uint32_t limb = 0; limb < 4; limb++) {
-    lk_gather_limb_kernel<<<nb(n), 256, 0, d.stream>>>(canon, idx_a, limb, keys_a, n);
+    SPB_TRY(launch(ctx, d.stream, nblk(n, 256), 256, 0, lk_gather_limb_kernel, canon, idx_a, limb, keys_a, n));
     SPB_TRY(radix_sort_pairs_u64(ctx, d, keys_a, keys_b, idx_a, idx_b, n, hist, tile_hist, tmp, tmp_bytes));   // result back in keys_a / idx_a
   }
-  lk_gather_kernel<<<nb(n), 256, 0, d.stream>>>(canon, idx_a, sorted, n);
-  ctx->n_kernel_launches += 6;
-  return 0;
+  return launch(ctx, d.stream, nblk(n, 256), 256, 0, lk_gather_kernel, canon, idx_a, sorted, n);
 }
 }  // namespace
 
@@ -197,9 +190,7 @@ int spb_permute_expression_pair_dev(spb_ctx* ctx, const spb_fr* d_input, const s
   if (!ctx || (usable && (!d_input || !d_table || !d_permuted_input || !d_permuted_table))) return SPB_ERR_ARG;
   if (!usable) return 0;
   if (usable >= 0x7fffffffull) return SPB_ERR_ARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  DeviceState& d = ctx->dev[0];
-  SPB_CUDA(ctx, cudaSetDevice(d.device));
+  SPB_ENTER(ctx);
   const uint64_t n = usable;
   Fr* canon = (Fr*)slot(ctx, d, "lk_canon", n * 32);
   Fr* sin = (Fr*)slot(ctx, d, "lk_sin", n * 32);
@@ -225,9 +216,9 @@ int spb_permute_expression_pair_dev(spb_ctx* ctx, const spb_fr* d_input, const s
   SPB_TRY(sort_canonical(ctx, d, (const Fr*)d_table, canon, stb, idx_a, idx_b, keys_a, keys_b, rs_hist, rs_tile, tmp, tmp_bytes, n));
   SPB_CUDA(ctx, cudaMemsetAsync(flags, 0, (4 * n + 8) * 4, d.stream));
   SPB_CUDA(ctx, cudaMemsetAsync(err, 0, 4, d.stream));
-  lk_match_kernel<<<nb(n), 256, 0, d.stream>>>(sin, stb, n, repeated_flag, used, err);
+  SPB_TRY(launch(ctx, d.stream, nblk(n, 256), 256, 0, lk_match_kernel, sin, stb, n, repeated_flag, used, err));
   SPB_CUDA(ctx, cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, repeated_flag, rep_rank, (int)n + 1, d.stream));   // rep_rank[n] = #repeated
-  lk_leftover_flag_kernel<<<nb(n), 256, 0, d.stream>>>(used, used, n);                                            // in place: used -> left_flag
+  SPB_TRY(launch(ctx, d.stream, nblk(n, 256), 256, 0, lk_leftover_flag_kernel, used, used, n));                   // in place: used -> left_flag
   SPB_CUDA(ctx, cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, used, left_rank, (int)n + 1, d.stream));            // left_rank[n] = #leftover
   uint32_t counts[2] = {0, 0}; int herr = 0;
   SPB_CUDA(ctx, cudaMemcpyAsync(&counts[0], rep_rank + n, 4, cudaMemcpyDeviceToHost, d.stream));
@@ -236,10 +227,8 @@ int spb_permute_expression_pair_dev(spb_ctx* ctx, const spb_fr* d_input, const s
   SPB_CUDA(ctx, cudaStreamSynchronize(d.stream));
   if (herr || counts[0] != counts[1]) return set_error(ctx, SPB_ERR_CONSTRAINT, "permute_expression_pair: an input value does not occur in the table (ConstraintSystemFailure)");
   uint32_t* rep_rows = idx_b;   // free again
-  lk_emit_input_kernel<<<nb(n), 256, 0, d.stream>>>(sin, repeated_flag, rep_rank, rep_rows, (Fr*)d_permuted_input, (Fr*)d_permuted_table, n);
-  lk_emit_leftover_kernel<<<nb(n), 256, 0, d.stream>>>(stb, used, left_rank, rep_rows, counts[0], (Fr*)d_permuted_table, n);
-  SPB_CUDA(ctx, cudaGetLastError());
-  ctx->n_kernel_launches += 4;
+  SPB_TRY(launch(ctx, d.stream, nblk(n, 256), 256, 0, lk_emit_input_kernel, sin, repeated_flag, rep_rank, rep_rows, (Fr*)d_permuted_input, (Fr*)d_permuted_table, n));
+  SPB_TRY(launch(ctx, d.stream, nblk(n, 256), 256, 0, lk_emit_leftover_kernel, stb, used, left_rank, rep_rows, counts[0], (Fr*)d_permuted_table, n));
   SPB_CUDA(ctx, cudaStreamSynchronize(d.stream));
   return 0;
 }

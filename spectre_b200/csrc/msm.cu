@@ -118,7 +118,7 @@ static int msm_enqueue(spb_ctx* ctx, DeviceState& d, int lane, Lane& ln, const F
   const unsigned tb = 256;
   SPB_CUDA(ctx, cudaMemsetAsync(counts, 0, (nb + 1) * 4, st));
   cudaEventRecord(ln.ev[0], st);
-  msm_count_kernel<<<(unsigned)((n + tb - 1) / tb), tb, 0, st>>>(n, d_scalars, g, counts);
+  SPB_TRY(launch(ctx, st, nblk(n, tb), tb, 0, msm_count_kernel, n, d_scalars, g, counts));
   cudaEventRecord(ln.ev[1], st);
   SPB_CUDA(ctx, cub::DeviceScan::ExclusiveSum(scan_tmp, scan_bytes, counts, offsets, (int)(nb + 1), st));
   // cursor := offsets (the counters are dead after the scan; reuse their storage)
@@ -126,24 +126,22 @@ static int msm_enqueue(spb_ctx* ctx, DeviceState& d, int lane, Lane& ln, const F
   cudaEventRecord(ln.ev[2], st);
   // (Two alternatives to this one-pass counting sort were built and measured slower at every size -- a second scatter pass with
   // L2-resident write windows, and a bin-local sort ranking in shared memory.)
-  msm_scatter_kernel<<<(unsigned)((n + tb - 1) / tb), tb, 0, st>>>(n, d_scalars, g, counts, ent);
+  SPB_TRY(launch(ctx, st, nblk(n, tb), tb, 0, msm_scatter_kernel, n, d_scalars, g, counts, ent));
   const uint32_t* total = offsets + nb;  // number of entries M, resident on the device
   cudaEventRecord(ln.ev[3], st);
-  msm_accumulate_kernel<<<(unsigned)((Tmax + 127) / 128), 128, 0, st>>>(total, g, ent, d_bases, buckets, head_key, head, tail_key, tail);
+  SPB_TRY(launch(ctx, st, nblk(Tmax, 128), 128, 0, msm_accumulate_kernel, total, g, ent, d_bases, buckets, head_key, head, tail_key, tail));
   cudaEventRecord(ln.ev[4], st);
-  msm_stitch_kernel<<<(unsigned)((Tmax + 127) / 128), 128, 0, st>>>(total, g.L, 24, head_key, head, tail_key, tail, buckets, giant, giant + 1);
-  msm_giant_kernel<<<256, 128, 0, st>>>(total, g.L, giant, giant + 1, head_key, head, tail_key, tail, buckets, huge, huge + 2);
-  msm_huge_kernel<<<kHugeBlocks, 128, 0, st>>>(huge, huge + 2, head, huge_part);
-  msm_huge_finish_kernel<<<64, 128, 0, st>>>(huge, huge + 2, kHugeBlocks, huge_part, tail_key, tail, buckets);
+  SPB_TRY(launch(ctx, st, nblk(Tmax, 128), 128, 0, msm_stitch_kernel, total, g.L, 24, head_key, head, tail_key, tail, buckets, giant, giant + 1));
+  SPB_TRY(launch(ctx, st, 256, 128, 0, msm_giant_kernel, total, g.L, giant, giant + 1, head_key, head, tail_key, tail, buckets, huge, huge + 2));
+  SPB_TRY(launch(ctx, st, kHugeBlocks, 128, 0, msm_huge_kernel, huge, huge + 2, head, huge_part));
+  SPB_TRY(launch(ctx, st, 64, 128, 0, msm_huge_finish_kernel, huge, huge + 2, kHugeBlocks, huge_part, tail_key, tail, buckets));
   cudaEventRecord(ln.ev[5], st);
   G1Xyzz *rows = seg_out, *cols = seg_out + (uint64_t)g.BW * R, *wrows = seg_out + (uint64_t)g.BW * (R + C);
-  msm_group_kernel<<<(unsigned)((ngroups + 127) / 128), 128, 0, st>>>(ngroups, tl.m_log, offsets, buckets, grp, grp + ngroups);
+  SPB_TRY(launch(ctx, st, nblk(ngroups, 128), 128, 0, msm_group_kernel, ngroups, tl.m_log, offsets, buckets, grp, grp + ngroups));
   cudaEventRecord(ln.ev[6], st);
-  msm_rowcol_kernel<<<g.BW * (2 * R + C), 64, 0, st>>>(T1, tl, grp, grp + ngroups, rows, cols, wrows);
-  msm_weighted_kernel<<<g.BW * (2 * tl.nbr + tl.nbc), 128, 0, st>>>(tl, rows, cols, wrows, win_out);
+  SPB_TRY(launch(ctx, st, g.BW * (2 * R + C), 64, 0, msm_rowcol_kernel, T1, tl, grp, grp + ngroups, rows, cols, wrows));
+  SPB_TRY(launch(ctx, st, g.BW * (2 * tl.nbr + tl.nbc), 128, 0, msm_weighted_kernel, tl, rows, cols, wrows, win_out));
   cudaEventRecord(ln.ev[7], st);
-  SPB_CUDA(ctx, cudaGetLastError());
-  ctx->n_kernel_launches += 10;
   SPB_CUDA(ctx, cudaMemcpyAsync(ln.pinned, win_out, (size_t)g.BW * per * sizeof(G1Xyzz), cudaMemcpyDeviceToHost, st));
   SPB_CUDA(ctx, cudaMemcpyAsync((char*)ln.pinned + (size_t)g.BW * per * sizeof(G1Xyzz), total, 4, cudaMemcpyDeviceToHost, st));
   return 0;
@@ -223,6 +221,11 @@ static int job_collect(spb_ctx* ctx, int lane, const std::vector<MsmPart>& parts
   ctx->last_kernel_ms = worst;
   write_result(acc, out);
   return 0;
+}
+
+// out[i] = scalars[i] * G1 generator, affine
+static int g1_fixed_base_mul(spb_ctx* ctx, DeviceState& d, const Fr* scalars, size_t n, G1Affine* out) {
+  return launch(ctx, d.stream, nblk(n, 128), 128, 0, g1_fixed_base_mul_kernel, scalars, n, out);
 }
 
 }  // namespace spb
@@ -326,10 +329,8 @@ int spb_srs_setup(spb_ctx* ctx, uint32_t k, const spb_fr* secret, spb_srs** out)
   {
     std::lock_guard<std::mutex> lk(ctx->mu);
     s = srs_alloc(ctx, k);
-    Fr tau; memcpy(&tau, secret, 32);
+    const Fr tau = fr_load(secret), w = fr_root_of_unity(k);
     const uint64_t n = 1ull << k;
-    Fr w; { constexpr uint32_t v[8] = SPB_FR_ROOT_OF_UNITY_MONT; for (int i = 0; i < 8; i++) w.l[i] = v[i]; }
-    for (uint32_t i = k; i < 28; i++) w = fp_sqr(w);
     Fr coef = fp_mul(fp_sub(fp_pow_u64(tau, n), fp_one<FrParams>()), fp_inv(fr_from_u64(n)));
     for (auto& sh : s->shards) {
       if (!sh.count) continue;
@@ -340,14 +341,13 @@ int spb_srs_setup(spb_ctx* ctx, uint32_t k, const spb_fr* secret, spb_srs** out)
       if (e == cudaSuccess) e = cudaMalloc(&sh.g, sh.count * sizeof(G1Affine));
       if (e == cudaSuccess) e = cudaMalloc(&sh.g_lagrange, sh.count * sizeof(G1Affine));
       if (e != cudaSuccess) { set_error(ctx, SPB_ERR_CUDA, "spb_srs_setup: %s", cudaGetErrorString(e)); goto fail; }
-      unsigned blocks = (unsigned)((sh.count + 127) / 128);
-      srs_scalars_kernel<<<blocks, 128, 0, d.stream>>>(0, tau, w, coef, sh.start, sh.count, sc);
-      g1_fixed_base_mul_kernel<<<blocks, 128, 0, d.stream>>>(sc, sh.count, sh.g);
-      srs_scalars_kernel<<<blocks, 128, 0, d.stream>>>(1, tau, w, coef, sh.start, sh.count, sc);
-      g1_fixed_base_mul_kernel<<<blocks, 128, 0, d.stream>>>(sc, sh.count, sh.g_lagrange);
-      ctx->n_kernel_launches += 4;
+      const unsigned blocks = nblk(sh.count, 128);
+      if (launch(ctx, d.stream, blocks, 128, 0, srs_scalars_kernel, 0, tau, w, coef, sh.start, sh.count, sc) ||
+          g1_fixed_base_mul(ctx, d, sc, sh.count, sh.g) ||
+          launch(ctx, d.stream, blocks, 128, 0, srs_scalars_kernel, 1, tau, w, coef, sh.start, sh.count, sc) ||
+          g1_fixed_base_mul(ctx, d, sc, sh.count, sh.g_lagrange))
+        goto fail;
       e = cudaStreamSynchronize(d.stream);
-      if (e == cudaSuccess) e = cudaGetLastError();
       if (e != cudaSuccess) { set_error(ctx, SPB_ERR_CUDA, "spb_srs_setup: %s", cudaGetErrorString(e)); goto fail; }
     }
     *out = s;
@@ -378,18 +378,14 @@ static int srs_downsize_locked(spb_ctx* ctx, const spb_srs* srs, uint32_t k, spb
     const size_t cnt = (n - sh.start) < sh.count ? (n - sh.start) : sh.count;
     SPB_CUDA(ctx, cudaMemcpyPeerAsync(g0 + sh.start, d.device, sh.g, ctx->dev[sh.dev_index].device, cnt * sizeof(G1Affine), d.stream));
   }
-  Fr w; { constexpr uint32_t v[8] = SPB_FR_ROOT_OF_UNITY_MONT; for (int i = 0; i < 8; i++) w.l[i] = v[i]; }
-  for (uint32_t i = k; i < 28; i++) w = fp_sqr(w);
-  const Fr w_inv = fp_inv(w), n_inv = fp_inv(fr_from_u64(n));
+  const Fr w_inv = fp_inv(fr_root_of_unity(k)), n_inv = fp_inv(fr_from_u64(n));
   const unsigned tb = 128;
-  ec_lift_kernel<<<(unsigned)((n + tb - 1) / tb), tb, 0, d.stream>>>(n, g0, pts);
+  SPB_TRY(launch(ctx, d.stream, nblk(n, tb), tb, 0, ec_lift_kernel, n, g0, pts));
   if (n >= 2) {
-    fr_powers_kernel<<<(unsigned)((n / 2 + 255) / 256), 256, 0, d.stream>>>(tw, w_inv, n / 2);
-    for (uint64_t half = n / 2; half >= 1; half >>= 1) ec_ntt_stage_kernel<<<(unsigned)((n / 2 + tb - 1) / tb), tb, 0, d.stream>>>(n, half, tw, pts);
+    SPB_TRY(launch(ctx, d.stream, nblk(n / 2, 256), 256, 0, fr_powers_kernel, tw, w_inv, n / 2));
+    for (uint64_t half = n / 2; half >= 1; half >>= 1) SPB_TRY(launch(ctx, d.stream, nblk(n / 2, tb), tb, 0, ec_ntt_stage_kernel, n, half, tw, pts));
   }
-  ec_ntt_finish_kernel<<<(unsigned)((n + tb - 1) / tb), tb, 0, d.stream>>>(n, k, n_inv, pts, lag);
-  SPB_CUDA(ctx, cudaGetLastError());
-  ctx->n_kernel_launches += 3 + k;
+  SPB_TRY(launch(ctx, d.stream, nblk(n, tb), tb, 0, ec_ntt_finish_kernel, n, k, n_inv, pts, lag));
   spb_srs* s = srs_alloc(ctx, k);
   *made = s;
   memcpy(s->g2, srs->g2, 128); memcpy(s->s_g2, srs->s_g2, 128);
@@ -452,10 +448,8 @@ static int srs_check_points(spb_ctx* ctx, DeviceState& d, const G1Affine* pts, s
   const uint64_t blocks = (count + tb - 1) / tb, cap = (uint64_t)(d.sm_count > 0 ? d.sm_count : 1) * 8;
   SPB_CUDA(ctx, cudaMemsetAsync(first, 0xff, sizeof(unsigned long long), d.stream));
   SPB_CUDA(ctx, cudaEventRecord(d.ev0, d.stream));
-  srs_check_kernel<<<(unsigned)(blocks < cap ? blocks : cap), tb, 0, d.stream>>>(pts, count, first);
-  SPB_CUDA(ctx, cudaGetLastError());
+  SPB_TRY(launch(ctx, d.stream, (unsigned)(blocks < cap ? blocks : cap), tb, 0, srs_check_kernel, pts, count, first));
   SPB_CUDA(ctx, cudaEventRecord(d.ev1, d.stream));
-  ctx->n_kernel_launches++;
   unsigned long long h = 0;
   SPB_CUDA(ctx, cudaMemcpyAsync(&h, first, sizeof h, cudaMemcpyDeviceToHost, d.stream));
   SPB_CUDA(ctx, cudaStreamSynchronize(d.stream));
@@ -705,10 +699,8 @@ int spb_srs_precompute(spb_ctx* ctx, spb_srs* srs) {
       cudaError_t e = cudaMalloc(&tab, (size_t)W * sh.count * sizeof(G1Affine));
       if (e != cudaSuccess) return set_error(ctx, SPB_ERR_OOM, "spb_srs_precompute: cudaMalloc(%zu): %s", (size_t)W * sh.count * sizeof(G1Affine), cudaGetErrorString(e));
       SPB_CUDA(ctx, cudaMemcpyAsync(tab, *slotp, sh.count * sizeof(G1Affine), cudaMemcpyDeviceToDevice, d.stream));
-      msm_precompute_kernel<<<(unsigned)((sh.count + 127) / 128), 128, 0, d.stream>>>(sh.count, c, W, tab);
-      ctx->n_kernel_launches++;
+      SPB_TRY(launch(ctx, d.stream, nblk(sh.count, 128), 128, 0, msm_precompute_kernel, sh.count, c, W, tab));
       SPB_CUDA(ctx, cudaStreamSynchronize(d.stream));
-      SPB_CUDA(ctx, cudaGetLastError());
       cudaFree(*slotp);
       *slotp = tab;
     }
@@ -719,19 +711,10 @@ int spb_srs_precompute(spb_ctx* ctx, spb_srs* srs) {
 
 int spb_g1_fixed_base_mul(spb_ctx* ctx, const spb_fr* scalars, size_t n, spb_g1_affine* out) {
   if (!ctx || !scalars || !out) return SPB_ERR_ARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  DeviceState& d = ctx->dev[0];
-  SPB_CUDA(ctx, cudaSetDevice(d.device));
-  Fr* ds = (Fr*)slot(ctx, d, "srs_scalars", n * sizeof(Fr));
-  G1Affine* dp = (G1Affine*)slot(ctx, d, "fbm_out", n * sizeof(G1Affine));
-  if (!ds || !dp) return SPB_ERR_OOM;
-  SPB_CUDA(ctx, cudaMemcpyAsync(ds, scalars, n * sizeof(Fr), cudaMemcpyHostToDevice, d.stream));
-  g1_fixed_base_mul_kernel<<<(unsigned)((n + 127) / 128), 128, 0, d.stream>>>(ds, n, dp);
-  SPB_CUDA(ctx, cudaGetLastError());
-  ctx->n_kernel_launches++;
-  SPB_CUDA(ctx, cudaMemcpyAsync(out, dp, n * sizeof(G1Affine), cudaMemcpyDeviceToHost, d.stream));
-  SPB_CUDA(ctx, cudaStreamSynchronize(d.stream));
-  return 0;
+  if (!n) return 0;
+  SPB_ENTER(ctx);
+  return run_staged(ctx, d, {{"srs_scalars", n * sizeof(Fr), scalars, nullptr}, {"fbm_out", n * sizeof(G1Affine), nullptr, out}},
+                    [&](void* const* p) { return g1_fixed_base_mul(ctx, d, (const Fr*)p[0], n, (G1Affine*)p[1]); });
 }
 
 }  // extern "C"

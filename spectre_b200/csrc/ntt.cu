@@ -26,20 +26,17 @@ static int get_tables(spb_ctx* ctx, DeviceState& d, uint32_t k, const Fr& omega,
   size_t nlo = (size_t)1 << h, nhi = (size_t)1 << (k - h);
   SPB_CUDA(ctx, cudaMalloc(&t.tw_lo, nlo * sizeof(Fr)));
   SPB_CUDA(ctx, cudaMalloc(&t.tw_hi, nhi * sizeof(Fr)));
-  fr_pow_table_kernel<<<(unsigned)((nlo + 127) / 128), 128, 0, d.stream>>>(t.tw_lo, omega, nlo, 0);
-  fr_pow_table_kernel<<<(unsigned)((nhi + 127) / 128), 128, 0, d.stream>>>(t.tw_hi, omega, nhi, h);
-  SPB_CUDA(ctx, cudaGetLastError());
-  ctx->n_kernel_launches += 2;
+  SPB_TRY(launch(ctx, d.stream, nblk(nlo, 128), 128, 0, fr_pow_table_kernel, t.tw_lo, omega, nlo, 0));
+  SPB_TRY(launch(ctx, d.stream, nblk(nhi, 128), 128, 0, fr_pow_table_kernel, t.tw_hi, omega, nhi, h));
   {
     size_t used = 0;
     for (auto& o : d.ntt_tables) if (o.tw_full) used += ((size_t)1 << o.k) * sizeof(Fr);
     size_t need = ((size_t)1 << k) * sizeof(Fr);
     if (k >= 12 && used + need <= kFullTableBudget && cudaMalloc(&t.tw_full, need) == cudaSuccess) {
-      fr_pow_table_kernel<<<(unsigned)((((size_t)1 << k) + 127) / 128), 128, 0, d.stream>>>(t.tw_full, omega, (uint64_t)1 << k, 0);
-      ctx->n_kernel_launches++;
+      SPB_TRY(launch(ctx, d.stream, nblk((uint64_t)1 << k, 128), 128, 0, fr_pow_table_kernel, t.tw_full, omega, (uint64_t)1 << k, 0));
     } else {
       t.tw_full = nullptr;
-      cudaGetLastError();
+      cudaGetLastError();  // the optional table's failed cudaMalloc must not be reported by the next launch check
     }
   }
   // a long-lived prover touches a handful of (k, omega) pairs; cap the cache anyway
@@ -68,10 +65,7 @@ static int launch_pass(spb_ctx* ctx, DeviceState& d, const NttPlan& plan, uint32
   // that co-resident persistent CTAs run their load/compute phases in lockstep and lose the overlap that
   // hardware-scheduled one-tile CTAs get for free, so large transforms launch one CTA per tile.
   if (k > 20) grid = L.tiles;
-  ntt_pass_kernel<<<(unsigned)grid, L.threads, L.smem, d.stream>>>(p);
-  SPB_CUDA(ctx, cudaGetLastError());
-  ctx->n_kernel_launches++;
-  return 0;
+  return launch(ctx, d.stream, (unsigned)grid, L.threads, L.smem, ntt_pass_kernel, p);
 }
 
 static int set_smem_attr(spb_ctx* ctx, DeviceState& d) {
@@ -168,9 +162,7 @@ int ntt_multi_host(spb_ctx* ctx, const Fr* in, Fr* out, uint32_t k, const Fr& om
       NttGatherArgs ga; memset(&ga, 0, sizeof ga);
       for (size_t qs = 0; qs < G; qs++) ga.peers[qs] = A[qs];
       ga.dst = B[qd]; ga.rows_loc = rows_loc; ga.lo_loc = lo_loc; ga.row_base = qd * rows_loc; ga.g_log = g;
-      ntt_gather_kernel<<<dd.sm_count * 8, 256, 0, dd.stream>>>(ga);
-      SPB_CUDA(ctx, cudaGetLastError());
-      ctx->n_kernel_launches++;
+      SPB_TRY(launch(ctx, dd.stream, dd.sm_count * 8, 256, 0, ntt_gather_kernel, ga));
     } else {
       for (size_t qs = 0; qs < G; qs++)
         SPB_CUDA(ctx, cudaMemcpy2DAsync(B[qd] + qs * lo_loc, lo_count * sizeof(Fr), A[qs] + qd * rows_loc * lo_loc, lo_loc * sizeof(Fr),

@@ -14,21 +14,6 @@
 
 using namespace spb;
 
-namespace {
-
-inline unsigned nblk(uint64_t n, unsigned t) { return (unsigned)((n + t - 1) / t); }
-inline Fr fr_load(const spb_fr* p) { Fr a; memcpy(&a, p, 32); return a; }
-inline Fr fr_const(const uint32_t (&v)[8]) { Fr a; for (int i = 0; i < 8; i++) a.l[i] = v[i]; return a; }
-inline Fr fr_delta() { constexpr uint32_t v[8] = SPB_FR_DELTA_MONT; return fr_const(v); }
-inline Fr fr_omega(uint32_t k) {
-  constexpr uint32_t v[8] = SPB_FR_ROOT_OF_UNITY_MONT;
-  Fr w = fr_const(v);
-  for (uint32_t i = k; i < SPB_FR_S; i++) w = fp_sqr(w);
-  return w;
-}
-
-}  // namespace
-
 // omega^i = omega^(256 * block) * omega^thread: one long power per block (thread 0), an 8-bit power per thread; the row
 // bodies are perm_terms_row / lookup_terms_row in quotient.cuh.
 // rows [row_lo, row_hi) of the column (row_lo a multiple of 256); num / den receive them at local index row - row_lo
@@ -73,8 +58,8 @@ __global__ void sub_small_kernel(Fr* a, SmallPoly s) {
 namespace {
 
 // z[0] = init, z[i+1] = z[i] * num[i] / den[i] over the n rows of one column, then the last n_blinds entries <- blinds and
-// *tail_out <- z[n - n_blinds - 1] (synchronises). `terms(d, lo, cnt, num, den)` enqueues on d.stream the kernel that writes the
-// cnt numerators / denominators of rows lo.. into the device-local buffers.
+// *tail_out <- z[n - n_blinds - 1] (synchronises). `terms(d, lo, cnt, num, den)` launches on d.stream the kernel that writes the
+// cnt numerators / denominators of rows lo.. into the device-local buffers, and returns its status.
 // One device: terms, chunked batch inversion, product pass, chunked scan. Several devices (row ranges): every device does the
 // same on its range in its own HBM, reading the column inputs from the first device over NVLink; the 32-byte range totals are the
 // ONE exchange (through the host: G - 1 field products give every range its seed); the seeded scans then write their slice of z
@@ -94,12 +79,9 @@ int fraction_product(spb_ctx* ctx, size_t n, const Terms& terms, const Fr& init,
     Fr* num = (Fr*)slot(ctx, d, "plonk_num", cnt * 32); Fr* den = (Fr*)slot(ctx, d, "plonk_den", cnt * 32);
     if (!num || !den) return SPB_ERR_OOM;
     nums[r] = num;
-    terms(d, ranges[r].lo, cnt, num, den);
-    SPB_CUDA(ctx, cudaGetLastError());
-    ctx->n_kernel_launches++;
+    SPB_TRY(terms(d, ranges[r].lo, cnt, num, den));
     SPB_TRY(dev_batch_invert(ctx, d, den, cnt));
-    frac_mul_kernel<<<nblk(cnt, 256), 256, 0, d.stream>>>(num, den, cnt);
-    ctx->n_kernel_launches++;
+    SPB_TRY(launch(ctx, d.stream, nblk(cnt, 256), 256, 0, frac_mul_kernel, num, den, cnt));
     if (G > 1) SPB_TRY(dev_product_enqueue(ctx, d, num, cnt, &dtot[r]));
   }
   // seeds: seed_0 = init, seed_r = seed_{r-1} * total_{r-1}
@@ -206,11 +188,6 @@ void shplonk_release(spb_shplonk* s) {
 
 extern "C" {
 
-#define SPB_ENTER(ctx)                          \
-  std::lock_guard<std::mutex> lk((ctx)->mu);    \
-  DeviceState& d = (ctx)->dev[0];               \
-  SPB_CUDA(ctx, cudaSetDevice(d.device));
-
 int spb_permutation_product_dev(spb_ctx* ctx, uint32_t k, const spb_fr* const* d_values, const spb_fr* const* d_sigma, uint32_t n_cols, uint32_t first_col,
                                 const spb_fr* beta, const spb_fr* gamma, const spb_fr* blinds, uint32_t n_blinds, spb_fr* last_z, spb_fr* d_z) {
   if (!ctx) return SPB_ERR_ARG;
@@ -221,11 +198,11 @@ int spb_permutation_product_dev(spb_ctx* ctx, uint32_t k, const spb_fr* const* d
   SPB_ENTER(ctx);
   PermTermArgs a;
   for (uint32_t c = 0; c < n_cols; c++) { a.values[c] = (const Fr*)d_values[c]; a.sigma[c] = (const Fr*)d_sigma[c]; }
-  a.n_cols = n_cols; a.beta = fr_load(beta); a.gamma = fr_load(gamma); a.delta = fr_delta(); a.omega = fr_omega(k);
+  a.n_cols = n_cols; a.beta = fr_load(beta); a.gamma = fr_load(gamma); a.delta = fr_delta(); a.omega = fr_root_of_unity(k);
   a.delta_start = fp_mul(a.beta, fp_pow_u64(a.delta, first_col));
   Fr tail;
   auto terms = [&](DeviceState& dv, size_t lo, size_t cnt, Fr* num, Fr* den) {
-    perm_terms_kernel<<<nblk(cnt, 256), 256, 0, dv.stream>>>(a, lo, lo + cnt, num, den);
+    return launch(ctx, dv.stream, nblk(cnt, 256), 256, 0, perm_terms_kernel, a, lo, lo + cnt, num, den);
   };
   SPB_TRY(fraction_product(ctx, n, terms, fr_load(last_z), blinds, n_blinds, (Fr*)d_z, &tail));
   memcpy(last_z, &tail, 32);
@@ -241,8 +218,8 @@ int spb_lookup_product_dev(spb_ctx* ctx, size_t n, const spb_fr* d_compressed_in
   SPB_ENTER(ctx);
   const Fr b = fr_load(beta), g = fr_load(gamma);
   auto terms = [&](DeviceState& dv, size_t lo, size_t cnt, Fr* num, Fr* den) {
-    lookup_terms_kernel<<<nblk(cnt, 256), 256, 0, dv.stream>>>((const Fr*)d_compressed_input + lo, (const Fr*)d_compressed_table + lo, (const Fr*)d_permuted_input + lo,
-                                                              (const Fr*)d_permuted_table + lo, b, g, cnt, num, den);
+    return launch(ctx, dv.stream, nblk(cnt, 256), 256, 0, lookup_terms_kernel, (const Fr*)d_compressed_input + lo, (const Fr*)d_compressed_table + lo,
+                  (const Fr*)d_permuted_input + lo, (const Fr*)d_permuted_table + lo, b, g, cnt, num, den);
   };
   return fraction_product(ctx, n, terms, fp_one<FrParams>(), blinds, n_blinds, (Fr*)d_z, nullptr);
 }
@@ -250,15 +227,14 @@ int spb_lookup_product_dev(spb_ctx* ctx, size_t n, const spb_fr* d_compressed_in
 int spb_weighted_sum_dev(spb_ctx* ctx, const spb_fr* const* d_polys, const spb_fr* weights, size_t count, spb_fr* d_out, size_t n) {
   if (!ctx) return SPB_ERR_ARG;
   if (!d_polys || !weights || !count || !d_out) return set_error(ctx, SPB_ERR_ARG, "spb_weighted_sum_dev: null argument");
+  if (!n) return 0;
   SPB_ENTER(ctx);
   char* buf = (char*)slot(ctx, d, "plonk_wsum", count * (sizeof(void*) + 32));
   if (!buf) return SPB_ERR_OOM;
   Fr* dw = (Fr*)buf; const Fr** dp = (const Fr**)(buf + count * 32);
   SPB_CUDA(ctx, cudaMemcpyAsync(dw, weights, count * 32, cudaMemcpyHostToDevice, d.stream));
   SPB_CUDA(ctx, cudaMemcpyAsync(dp, d_polys, count * sizeof(void*), cudaMemcpyHostToDevice, d.stream));
-  weighted_sum_kernel<<<nblk(n, 256), 256, 0, d.stream>>>(dp, dw, (uint32_t)count, (Fr*)d_out, n);
-  SPB_CUDA(ctx, cudaGetLastError());
-  ctx->n_kernel_launches++;
+  SPB_TRY(launch(ctx, d.stream, nblk(n, 256), 256, 0, weighted_sum_kernel, dp, dw, (uint32_t)count, (Fr*)d_out, n));
   SPB_CUDA(ctx, cudaStreamSynchronize(d.stream));
   return 0;
 }
@@ -346,9 +322,8 @@ int spb_shplonk_begin_dev(spb_ctx* ctx, const spb_srs* srs, size_t n, const spb_
       for (uint32_t t = 0; t < np; t++) rsum.c[t] = fp_zero<FrParams>();
       for (uint32_t j = 0; j < m; j++) for (uint32_t t = 0; t < np; t++) rsum.c[t] = fp_add(rsum.c[t], fp_mul(w[j], st.r[j][t]));
       SHP_CUDA(cudaMemcpyAsync(s->d_w + base, w.data(), (size_t)m * 32, cudaMemcpyHostToDevice, d.stream));
-      weighted_sum_kernel<<<nblk(n, 256), 256, 0, d.stream>>>(s->d_ptrs + base, s->d_w + base, m, s->d_tmp[0], n);
-      sub_small_kernel<<<1, 8, 0, d.stream>>>(s->d_tmp[0], rsum);
-      ctx->n_kernel_launches += 2;
+      if ((rc = launch(ctx, d.stream, nblk(n, 256), 256, 0, weighted_sum_kernel, s->d_ptrs + base, s->d_w + base, m, s->d_tmp[0], n)) != 0) return fail(rc);
+      if ((rc = launch(ctx, d.stream, 1, 8, 0, sub_small_kernel, s->d_tmp[0], rsum)) != 0) return fail(rc);
       // Q_i(X) = N_i(X) / prod_p (X - point_p): one Kate division per point
       size_t len = n; int cur = 0;
       for (uint32_t p = 0; p < np; p++) {
@@ -356,13 +331,11 @@ int spb_shplonk_begin_dev(spb_ctx* ctx, const spb_srs* srs, size_t n, const spb_
         cur ^= 1; len--;
       }
       // h <- h + v^i * Q_i (Q_i zero-extended to n)   (upstream: quotient_polynomials.zip(powers(v)))
-      scale_add_kernel<<<nblk(n, 256), 256, 0, d.stream>>>(s->d_h, fp_one<FrParams>(), s->d_tmp[cur], vpow, len, n);
+      if ((rc = launch(ctx, d.stream, nblk(n, 256), 256, 0, scale_add_kernel, s->d_h, fp_one<FrParams>(), s->d_tmp[cur], vpow, len, n)) != 0) return fail(rc);
       vpow = fp_mul(vpow, s->v);
-      ctx->n_kernel_launches++;
       SHP_CUDA(cudaStreamSynchronize(d.stream));   // w (host vector) must outlive the copy
       base += m;
     }
-    SHP_CUDA(cudaGetLastError());
   }
   rc = spb_msm_dev(ctx, srs, SPB_BASIS_G, (const spb_fr*)s->d_h, n, h_commitment);
   if (rc != 0) { std::lock_guard<std::mutex> lk(ctx->mu); shplonk_release(s); return rc; }
@@ -409,17 +382,14 @@ int spb_shplonk_finish_dev(spb_ctx* ctx, spb_shplonk* s, const spb_fr* u, spb_g1
     SHP_CUDA(cudaSetDevice(d.device));
     SHP_CUDA(cudaMemcpyAsync(s->d_w, w.data(), (size_t)s->n_polys * 32, cudaMemcpyHostToDevice, d.stream));
     // L(X) = sum w_ij P_ij(X) - constant - Z_T(u) h(X)
-    weighted_sum_kernel<<<nblk(n, 256), 256, 0, d.stream>>>(s->d_ptrs, s->d_w, s->n_polys, s->d_tmp[0], n);
+    if ((rc = launch(ctx, d.stream, nblk(n, 256), 256, 0, weighted_sum_kernel, s->d_ptrs, s->d_w, s->n_polys, s->d_tmp[0], n)) != 0) return fail(rc);
     SmallPoly c0; c0.n = 1; c0.c[0] = constant;
-    sub_small_kernel<<<1, 8, 0, d.stream>>>(s->d_tmp[0], c0);
+    if ((rc = launch(ctx, d.stream, 1, 8, 0, sub_small_kernel, s->d_tmp[0], c0)) != 0) return fail(rc);
     // tmp0 <- 1 * tmp0 + (-zt) * h  ==  scale_add on a copy of h: h <- (-zt) * h + tmp0
-    scale_add_kernel<<<nblk(n, 256), 256, 0, d.stream>>>(s->d_h, fp_neg(zt), s->d_tmp[0], fp_one<FrParams>(), n, n);
-    ctx->n_kernel_launches += 3;
+    if ((rc = launch(ctx, d.stream, nblk(n, 256), 256, 0, scale_add_kernel, s->d_h, fp_neg(zt), s->d_tmp[0], fp_one<FrParams>(), n, n)) != 0) return fail(rc);
     // (L(X) / (X - u)) / Z_{T \ S_0}(u)
     if ((rc = dev_kate_division(ctx, d, s->d_h, n, uu, s->d_tmp[1])) != 0) return fail(rc);
-    scale_add_kernel<<<nblk(n - 1, 256), 256, 0, d.stream>>>(s->d_tmp[1], z0_inv, nullptr, fp_zero<FrParams>(), 0, n - 1);
-    ctx->n_kernel_launches++;
-    SHP_CUDA(cudaGetLastError());
+    if ((rc = launch(ctx, d.stream, nblk(n - 1, 256), 256, 0, scale_add_kernel, s->d_tmp[1], z0_inv, nullptr, fp_zero<FrParams>(), 0, n - 1)) != 0) return fail(rc);
     SHP_CUDA(cudaStreamSynchronize(d.stream));
   }
   rc = spb_msm_dev(ctx, s->srs, SPB_BASIS_G, (const spb_fr*)s->d_tmp[1], n - 1, commitment);

@@ -162,10 +162,11 @@ __global__ void inv_partials_kernel(Fr* partial, uint64_t m) {
 }
 
 // ---- polynomial evaluation: p(x) = sum_t x^t * q_t(x^T), q_t = coefficients t, t+T, ... (coalesced Horner) ------
-// T threads in blocks of 256; each block folds its 256 terms with a shared-memory tree and writes one partial.
-__global__ void __launch_bounds__(256) eval_strided_kernel(const Fr* poly, uint64_t n, Fr x, Fr xT, uint32_t T, Fr* partial) {
+// T threads in blocks of 256; thread t runs the Horner of q_t, the block folds its 256 terms with a shared-memory tree. The
+// block's partial sum is valid in thread 0.
+__device__ __forceinline__ Fr eval_block_partial(const Fr* poly, uint64_t n, Fr x, Fr xT, uint32_t T) {
   __shared__ Fr sh[128];
-  uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
   Fr acc = fp_zero<FrParams>();
   if (t < T && t < n) {
     uint64_t last = t + ((n - 1 - t) / T) * T;
@@ -178,29 +179,17 @@ __global__ void __launch_bounds__(256) eval_strided_kernel(const Fr* poly, uint6
     if ((int)threadIdx.x < stride) acc = fp_add(acc, sh[threadIdx.x]);
     __syncthreads();
   }
+  return acc;
+}
+__global__ void __launch_bounds__(256) eval_strided_kernel(const Fr* poly, uint64_t n, Fr x, Fr xT, uint32_t T, Fr* partial) {
+  Fr acc = eval_block_partial(poly, n, x, xT, T);
   if (threadIdx.x == 0) partial[blockIdx.x] = acc;
 }
-
-
 // the same for a whole list of (polynomial, point) queries in ONE launch: blockIdx.y = query (create_proof evaluates every
 // opened polynomial at every queried rotation after squeezing x: 153 queries in the sync-step shape)
 __global__ void __launch_bounds__(256) eval_many_kernel(const Fr* const* polys, const Fr* xs /* (x, x^T) per query */, uint64_t n, uint32_t T, Fr* partial) {
-  __shared__ Fr sh[128];
-  const uint32_t q = blockIdx.y, t = blockIdx.x * blockDim.x + threadIdx.x;
-  const Fr* poly = polys[q];
-  const Fr x = xs[2 * q], xT = xs[2 * q + 1];
-  Fr acc = fp_zero<FrParams>();
-  if (t < T && t < n) {
-    uint64_t last = t + ((n - 1 - t) / T) * T;
-    for (uint64_t i = last;; i -= T) { acc = fp_add(fp_mul(acc, xT), ntt_ldg(poly + i)); if (i < T) break; }
-    acc = fp_mul(acc, fp_pow_u64(x, t));
-  }
-  for (int stride = 128; stride >= 1; stride >>= 1) {
-    if ((int)threadIdx.x >= stride && (int)threadIdx.x < 2 * stride) sh[threadIdx.x - stride] = acc;
-    __syncthreads();
-    if ((int)threadIdx.x < stride) acc = fp_add(acc, sh[threadIdx.x]);
-    __syncthreads();
-  }
+  const uint32_t q = blockIdx.y;
+  Fr acc = eval_block_partial(polys[q], n, xs[2 * q], xs[2 * q + 1], T);
   if (threadIdx.x == 0) partial[(uint64_t)q * gridDim.x + blockIdx.x] = acc;
 }
 
@@ -216,19 +205,24 @@ __global__ void lincomb_kernel(const Fr* const* polys, uint32_t count, Fr y, Fr*
 
 namespace spb {
 
-static inline unsigned nblk(uint64_t n, unsigned t) { return (unsigned)((n + t - 1) / t); }
-
 // ---- device-resident cores (all pointers on device d, work enqueued on d.stream; no final synchronisation unless noted)
+static int dev_vec_mul(spb_ctx* ctx, DeviceState& d, Fr* da, const Fr* db, size_t n) {
+  return launch(ctx, d.stream, nblk(n, 256), 256, 0, vec_mul_kernel, da, db, n);
+}
+static int dev_vec_axpy(spb_ctx* ctx, DeviceState& d, Fr* dy, const Fr& alpha, const Fr* dx, size_t n) {
+  return launch(ctx, d.stream, nblk(n, 256), 256, 0, vec_axpy_kernel, dy, alpha, dx, n);
+}
+static int dev_vec_scale(spb_ctx* ctx, DeviceState& d, Fr* da, const Fr& alpha, size_t n) {
+  return launch(ctx, d.stream, nblk(n, 256), 256, 0, vec_scale_kernel, da, alpha, n);
+}
+
 int dev_grand_product(spb_ctx* ctx, DeviceState& d, const Fr* da, size_t n, Fr* dz, const Fr& init) {
   size_t m = (n + kScanChunk - 1) / kScanChunk;
   Fr* dp = (Fr*)slot(ctx, d, "poly_partial", 2 * m * 32);
   if (!dp) return SPB_ERR_OOM;
-  chunk_product_kernel<<<nblk(m, 128), 128, 0, d.stream>>>(da, n, dp);
-  carry_product_kernel<<<1, 1024, 0, d.stream>>>(dp, m);
-  chunk_product_fix_kernel<<<nblk(m, 128), 128, 0, d.stream>>>(da, n, dp, init, dz);
-  SPB_CUDA(ctx, cudaGetLastError());
-  ctx->n_kernel_launches += 3;
-  return 0;
+  SPB_TRY(launch(ctx, d.stream, nblk(m, 128), 128, 0, chunk_product_kernel, da, n, dp));
+  SPB_TRY(launch(ctx, d.stream, 1, 1024, 0, carry_product_kernel, dp, m));
+  return launch(ctx, d.stream, nblk(m, 128), 128, 0, chunk_product_fix_kernel, da, n, dp, init, dz);
 }
 
 // product of da[0..n) -> *d_total (one Fr in device memory of d, in the slot "poly_total"); enqueue only
@@ -237,10 +231,8 @@ int dev_product_enqueue(spb_ctx* ctx, DeviceState& d, const Fr* da, size_t n, Fr
   Fr* dp = (Fr*)slot(ctx, d, "poly_partial", 2 * m * 32);
   Fr* dt = (Fr*)slot(ctx, d, "poly_total", 32);
   if (!dp || !dt) return SPB_ERR_OOM;
-  chunk_product_kernel<<<nblk(m, 128), 128, 0, d.stream>>>(da, n, dp);
-  total_product_kernel<<<1, 1024, 0, d.stream>>>(dp, m, dt);
-  SPB_CUDA(ctx, cudaGetLastError());
-  ctx->n_kernel_launches += 2;
+  SPB_TRY(launch(ctx, d.stream, nblk(m, 128), 128, 0, chunk_product_kernel, da, n, dp));
+  SPB_TRY(launch(ctx, d.stream, 1, 1024, 0, total_product_kernel, dp, m, dt));
   *d_total = dt;
   return 0;
 }
@@ -249,13 +241,10 @@ int dev_kate_division(spb_ctx* ctx, DeviceState& d, const Fr* da, size_t n, cons
   size_t nq = n - 1, m = (nq + kScanChunk - 1) / kScanChunk;
   Fr* dh = (Fr*)slot(ctx, d, "poly_partial", 2 * m * 32);
   if (!dh) return SPB_ERR_OOM;
-  kate_chunk_kernel<<<nblk(m, 128), 128, 0, d.stream>>>(da, nq, bb, nullptr, dh, nullptr, 0);
+  SPB_TRY(launch(ctx, d.stream, nblk(m, 128), 128, 0, kate_chunk_kernel, da, nq, bb, nullptr, dh, nullptr, 0));
   size_t last_len = nq - (m - 1) * kScanChunk;
-  carry_kate_kernel<<<1, 512, 0, d.stream>>>(dh, dh + m, m, fp_pow_u64(bb, kScanChunk), fp_pow_u64(bb, last_len));
-  kate_chunk_kernel<<<nblk(m, 128), 128, 0, d.stream>>>(da, nq, bb, dh + m, nullptr, dq, 1);
-  SPB_CUDA(ctx, cudaGetLastError());
-  ctx->n_kernel_launches += 3;
-  return 0;
+  SPB_TRY(launch(ctx, d.stream, 1, 512, 0, carry_kate_kernel, dh, dh + m, m, fp_pow_u64(bb, kScanChunk), fp_pow_u64(bb, last_len)));
+  return launch(ctx, d.stream, nblk(m, 128), 128, 0, kate_chunk_kernel, da, nq, bb, dh + m, nullptr, dq, 1);
 }
 
 int dev_batch_invert(spb_ctx* ctx, DeviceState& d, Fr* da, size_t n) {
@@ -263,11 +252,9 @@ int dev_batch_invert(spb_ctx* ctx, DeviceState& d, Fr* da, size_t n) {
   Fr* ds = (Fr*)slot(ctx, d, "poly_scratch", n * 32);
   Fr* dp = (Fr*)slot(ctx, d, "poly_partial", 2 * m * 32);
   if (!ds || !dp) return SPB_ERR_OOM;
-  inv_chunk_prefix_kernel<<<nblk(m, 64), 64, 0, d.stream>>>(da, n, ds, dp);
-  inv_partials_kernel<<<nblk(m, 64), 64, 0, d.stream>>>(dp, m);
-  inv_chunk_fix_kernel<<<nblk(m, 64), 64, 0, d.stream>>>(da, n, ds, dp);
-  ctx->n_kernel_launches += 3;
-  return 0;
+  SPB_TRY(launch(ctx, d.stream, nblk(m, 64), 64, 0, inv_chunk_prefix_kernel, da, n, ds, dp));
+  SPB_TRY(launch(ctx, d.stream, nblk(m, 64), 64, 0, inv_partials_kernel, dp, m));
+  return launch(ctx, d.stream, nblk(m, 64), 64, 0, inv_chunk_fix_kernel, da, n, ds, dp);
 }
 
 int dev_eval_polynomial(spb_ctx* ctx, DeviceState& d, const Fr* dp, size_t n, const Fr& x, Fr* out_host) {
@@ -277,8 +264,7 @@ int dev_eval_polynomial(spb_ctx* ctx, DeviceState& d, const Fr* dp, size_t n, co
   const uint32_t blocks = T / 256;
   Fr* dpart = (Fr*)slot(ctx, d, "poly_partial", (size_t)blocks * 32 > 64 ? (size_t)blocks * 32 : 64);
   if (!dpart) return SPB_ERR_OOM;
-  eval_strided_kernel<<<blocks, 256, 0, d.stream>>>(dp, n, x, fp_pow_u64(x, T), T, dpart);
-  ctx->n_kernel_launches++;
+  SPB_TRY(launch(ctx, d.stream, blocks, 256, 0, eval_strided_kernel, dp, n, x, fp_pow_u64(x, T), T, dpart));
   std::vector<Fr> part(blocks);
   SPB_CUDA(ctx, cudaMemcpyAsync(part.data(), dpart, (size_t)blocks * 32, cudaMemcpyDeviceToHost, d.stream));
   SPB_CUDA(ctx, cudaStreamSynchronize(d.stream));
@@ -333,90 +319,62 @@ __global__ void fr_random_chacha_kernel(ChaChaKey key, uint64_t first, uint64_t 
 
 extern "C" {
 
-#define SPB_ENTER(ctx)                          \
-  std::lock_guard<std::mutex> lk((ctx)->mu);    \
-  DeviceState& d = (ctx)->dev[0];               \
-  SPB_CUDA(ctx, cudaSetDevice(d.device));
-
 // ---- element-wise -------------------------------------------------------------------------------------------------
 int spb_vec_mul_dev(spb_ctx* ctx, spb_fr* d_a, const spb_fr* d_b, size_t n) {
   if (!ctx || !d_a || !d_b) return SPB_ERR_ARG;
+  if (!n) return 0;
   SPB_ENTER(ctx);
-  vec_mul_kernel<<<nblk(n, 256), 256, 0, d.stream>>>((Fr*)d_a, (const Fr*)d_b, n);
-  ctx->n_kernel_launches++;
+  SPB_TRY(dev_vec_mul(ctx, d, (Fr*)d_a, (const Fr*)d_b, n));
   SPB_CUDA(ctx, cudaStreamSynchronize(d.stream));
   return 0;
 }
 int spb_vec_axpy_dev(spb_ctx* ctx, spb_fr* d_y, const spb_fr* alpha, const spb_fr* d_x, size_t n) {
   if (!ctx || !d_y || !alpha || !d_x) return SPB_ERR_ARG;
+  if (!n) return 0;
   SPB_ENTER(ctx);
-  Fr al; memcpy(&al, alpha, 32);
-  vec_axpy_kernel<<<nblk(n, 256), 256, 0, d.stream>>>((Fr*)d_y, al, (const Fr*)d_x, n);
-  ctx->n_kernel_launches++;
+  SPB_TRY(dev_vec_axpy(ctx, d, (Fr*)d_y, fr_load(alpha), (const Fr*)d_x, n));
   SPB_CUDA(ctx, cudaStreamSynchronize(d.stream));
   return 0;
 }
 int spb_vec_scale_dev(spb_ctx* ctx, spb_fr* d_a, const spb_fr* alpha, size_t n) {
   if (!ctx || !d_a || !alpha) return SPB_ERR_ARG;
+  if (!n) return 0;
   SPB_ENTER(ctx);
-  Fr al; memcpy(&al, alpha, 32);
-  vec_scale_kernel<<<nblk(n, 256), 256, 0, d.stream>>>((Fr*)d_a, al, n);
-  ctx->n_kernel_launches++;
+  SPB_TRY(dev_vec_scale(ctx, d, (Fr*)d_a, fr_load(alpha), n));
   SPB_CUDA(ctx, cudaStreamSynchronize(d.stream));
   return 0;
 }
 int spb_lincomb_dev(spb_ctx* ctx, const spb_fr* const* d_polys, size_t count, const spb_fr* y, spb_fr* d_out, size_t n) {
   if (!ctx || !d_polys || !count || !y || !d_out) return SPB_ERR_ARG;
+  if (!n) return 0;
   SPB_ENTER(ctx);
   const Fr** dptrs = (const Fr**)slot(ctx, d, "poly_ptrs", count * sizeof(void*));
   if (!dptrs) return SPB_ERR_OOM;
   SPB_CUDA(ctx, cudaMemcpyAsync(dptrs, d_polys, count * sizeof(void*), cudaMemcpyHostToDevice, d.stream));
-  Fr yy; memcpy(&yy, y, 32);
-  lincomb_kernel<<<nblk(n, 256), 256, 0, d.stream>>>(dptrs, (uint32_t)count, yy, (Fr*)d_out, n);
-  ctx->n_kernel_launches++;
+  SPB_TRY(launch(ctx, d.stream, nblk(n, 256), 256, 0, lincomb_kernel, dptrs, (uint32_t)count, fr_load(y), (Fr*)d_out, n));
   SPB_CUDA(ctx, cudaStreamSynchronize(d.stream));
   return 0;
 }
 
 int spb_vec_mul(spb_ctx* ctx, spb_fr* a, const spb_fr* b, size_t n) {
   if (!ctx || !a || !b) return SPB_ERR_ARG;
+  if (!n) return 0;
   SPB_ENTER(ctx);
-  Fr* da = (Fr*)slot(ctx, d, "poly_a", n * 32); Fr* db = (Fr*)slot(ctx, d, "poly_b", n * 32);
-  if (!da || !db) return SPB_ERR_OOM;
-  SPB_CUDA(ctx, cudaMemcpyAsync(da, a, n * 32, cudaMemcpyHostToDevice, d.stream));
-  SPB_CUDA(ctx, cudaMemcpyAsync(db, b, n * 32, cudaMemcpyHostToDevice, d.stream));
-  vec_mul_kernel<<<nblk(n, 256), 256, 0, d.stream>>>(da, db, n);
-  ctx->n_kernel_launches++;
-  SPB_CUDA(ctx, cudaMemcpyAsync(a, da, n * 32, cudaMemcpyDeviceToHost, d.stream));
-  SPB_CUDA(ctx, cudaStreamSynchronize(d.stream));
-  return 0;
+  return run_staged(ctx, d, {{"poly_a", n * 32, a, a}, {"poly_b", n * 32, b, nullptr}},
+                    [&](void* const* p) { return dev_vec_mul(ctx, d, (Fr*)p[0], (const Fr*)p[1], n); });
 }
 int spb_vec_axpy(spb_ctx* ctx, spb_fr* y, const spb_fr* alpha, const spb_fr* x, size_t n) {
   if (!ctx || !y || !alpha || !x) return SPB_ERR_ARG;
+  if (!n) return 0;
   SPB_ENTER(ctx);
-  Fr* dy = (Fr*)slot(ctx, d, "poly_a", n * 32); Fr* dx = (Fr*)slot(ctx, d, "poly_b", n * 32);
-  if (!dy || !dx) return SPB_ERR_OOM;
-  Fr al; memcpy(&al, alpha, 32);
-  SPB_CUDA(ctx, cudaMemcpyAsync(dy, y, n * 32, cudaMemcpyHostToDevice, d.stream));
-  SPB_CUDA(ctx, cudaMemcpyAsync(dx, x, n * 32, cudaMemcpyHostToDevice, d.stream));
-  vec_axpy_kernel<<<nblk(n, 256), 256, 0, d.stream>>>(dy, al, dx, n);
-  ctx->n_kernel_launches++;
-  SPB_CUDA(ctx, cudaMemcpyAsync(y, dy, n * 32, cudaMemcpyDeviceToHost, d.stream));
-  SPB_CUDA(ctx, cudaStreamSynchronize(d.stream));
-  return 0;
+  return run_staged(ctx, d, {{"poly_a", n * 32, y, y}, {"poly_b", n * 32, x, nullptr}},
+                    [&](void* const* p) { return dev_vec_axpy(ctx, d, (Fr*)p[0], fr_load(alpha), (const Fr*)p[1], n); });
 }
 int spb_vec_scale(spb_ctx* ctx, spb_fr* a, const spb_fr* alpha, size_t n) {
   if (!ctx || !a || !alpha) return SPB_ERR_ARG;
+  if (!n) return 0;
   SPB_ENTER(ctx);
-  Fr* da = (Fr*)slot(ctx, d, "poly_a", n * 32);
-  if (!da) return SPB_ERR_OOM;
-  Fr al; memcpy(&al, alpha, 32);
-  SPB_CUDA(ctx, cudaMemcpyAsync(da, a, n * 32, cudaMemcpyHostToDevice, d.stream));
-  vec_scale_kernel<<<nblk(n, 256), 256, 0, d.stream>>>(da, al, n);
-  ctx->n_kernel_launches++;
-  SPB_CUDA(ctx, cudaMemcpyAsync(a, da, n * 32, cudaMemcpyDeviceToHost, d.stream));
-  SPB_CUDA(ctx, cudaStreamSynchronize(d.stream));
-  return 0;
+  return run_staged(ctx, d, {{"poly_a", n * 32, a, a}}, [&](void* const* p) { return dev_vec_scale(ctx, d, (Fr*)p[0], fr_load(alpha), n); });
 }
 
 // ---- scans --------------------------------------------------------------------------------------------------------
@@ -432,21 +390,15 @@ int spb_grand_product(spb_ctx* ctx, const spb_fr* a, size_t n, spb_fr* z) {
   if (!ctx || !a || !z) return SPB_ERR_ARG;
   if (!n) return 0;
   SPB_ENTER(ctx);
-  Fr* da = (Fr*)slot(ctx, d, "poly_a", n * 32); Fr* dz = (Fr*)slot(ctx, d, "poly_b", n * 32);
-  if (!da || !dz) return SPB_ERR_OOM;
-  SPB_CUDA(ctx, cudaMemcpyAsync(da, a, n * 32, cudaMemcpyHostToDevice, d.stream));
-  SPB_TRY(dev_grand_product(ctx, d, da, n, dz, fp_one<FrParams>()));
-  SPB_CUDA(ctx, cudaMemcpyAsync(z, dz, n * 32, cudaMemcpyDeviceToHost, d.stream));
-  SPB_CUDA(ctx, cudaStreamSynchronize(d.stream));
-  return 0;
+  return run_staged(ctx, d, {{"poly_a", n * 32, a, nullptr}, {"poly_b", n * 32, nullptr, z}},
+                    [&](void* const* p) { return dev_grand_product(ctx, d, (const Fr*)p[0], n, (Fr*)p[1], fp_one<FrParams>()); });
 }
 
 int spb_grand_product_seeded_dev(spb_ctx* ctx, const spb_fr* d_a, size_t n, const spb_fr* init, spb_fr* d_z) {
   if (!ctx || !d_a || !d_z || !init) return SPB_ERR_ARG;
   if (!n) return 0;
   SPB_ENTER(ctx);
-  Fr seed; memcpy(&seed, init, 32);
-  SPB_TRY(dev_grand_product(ctx, d, (const Fr*)d_a, n, (Fr*)d_z, seed));
+  SPB_TRY(dev_grand_product(ctx, d, (const Fr*)d_a, n, (Fr*)d_z, fr_load(init)));
   SPB_CUDA(ctx, cudaStreamSynchronize(d.stream));
   return 0;
 }
@@ -468,8 +420,7 @@ int spb_kate_division_dev(spb_ctx* ctx, const spb_fr* d_a, size_t n, const spb_f
   if (!ctx || !d_a || !b || !d_q || n < 1) return SPB_ERR_ARG;
   if (n == 1) return 0;
   SPB_ENTER(ctx);
-  Fr bb; memcpy(&bb, b, 32);
-  SPB_TRY(dev_kate_division(ctx, d, (const Fr*)d_a, n, bb, (Fr*)d_q));
+  SPB_TRY(dev_kate_division(ctx, d, (const Fr*)d_a, n, fr_load(b), (Fr*)d_q));
   SPB_CUDA(ctx, cudaStreamSynchronize(d.stream));
   return 0;
 }
@@ -477,14 +428,8 @@ int spb_kate_division(spb_ctx* ctx, const spb_fr* a, size_t n, const spb_fr* b, 
   if (!ctx || !a || !b || !q || n < 1) return SPB_ERR_ARG;
   if (n == 1) return 0;
   SPB_ENTER(ctx);
-  Fr* da = (Fr*)slot(ctx, d, "poly_a", n * 32); Fr* dq = (Fr*)slot(ctx, d, "poly_b", n * 32);
-  if (!da || !dq) return SPB_ERR_OOM;
-  Fr bb; memcpy(&bb, b, 32);
-  SPB_CUDA(ctx, cudaMemcpyAsync(da, a, n * 32, cudaMemcpyHostToDevice, d.stream));
-  SPB_TRY(dev_kate_division(ctx, d, da, n, bb, dq));
-  SPB_CUDA(ctx, cudaMemcpyAsync(q, dq, (n - 1) * 32, cudaMemcpyDeviceToHost, d.stream));
-  SPB_CUDA(ctx, cudaStreamSynchronize(d.stream));
-  return 0;
+  return run_staged(ctx, d, {{"poly_a", n * 32, a, nullptr}, {"poly_b", n * 32, nullptr, q, 0, (n - 1) * 32}},
+                    [&](void* const* p) { return dev_kate_division(ctx, d, (const Fr*)p[0], n, fr_load(b), (Fr*)p[1]); });
 }
 
 int spb_batch_invert_dev(spb_ctx* ctx, spb_fr* d_a, size_t n) {
@@ -499,13 +444,7 @@ int spb_batch_invert(spb_ctx* ctx, spb_fr* a, size_t n) {
   if (!ctx || !a) return SPB_ERR_ARG;
   if (!n) return 0;
   SPB_ENTER(ctx);
-  Fr* da = (Fr*)slot(ctx, d, "poly_a", n * 32);
-  if (!da) return SPB_ERR_OOM;
-  SPB_CUDA(ctx, cudaMemcpyAsync(da, a, n * 32, cudaMemcpyHostToDevice, d.stream));
-  SPB_TRY(dev_batch_invert(ctx, d, da, n));
-  SPB_CUDA(ctx, cudaMemcpyAsync(a, da, n * 32, cudaMemcpyDeviceToHost, d.stream));
-  SPB_CUDA(ctx, cudaStreamSynchronize(d.stream));
-  return 0;
+  return run_staged(ctx, d, {{"poly_a", n * 32, a, a}}, [&](void* const* p) { return dev_batch_invert(ctx, d, (Fr*)p[0], n); });
 }
 
 int spb_eval_polynomial_dev(spb_ctx* ctx, const spb_fr* d_poly, size_t n, const spb_fr* point, spb_fr* out) {
@@ -513,8 +452,7 @@ int spb_eval_polynomial_dev(spb_ctx* ctx, const spb_fr* d_poly, size_t n, const 
   Fr acc = fp_zero<FrParams>();
   if (n) {
     SPB_ENTER(ctx);
-    Fr x; memcpy(&x, point, 32);
-    SPB_TRY(dev_eval_polynomial(ctx, d, (const Fr*)d_poly, n, x, &acc));
+    SPB_TRY(dev_eval_polynomial(ctx, d, (const Fr*)d_poly, n, fr_load(point), &acc));
   }
   memcpy(out, &acc, 32);
   return 0;
@@ -532,12 +470,10 @@ int spb_eval_polynomial_many_dev(spb_ctx* ctx, const spb_fr* const* d_polys, siz
   Fr* dpart = (Fr*)slot(ctx, d, "evm_partial", count * blocks * sizeof(Fr));
   if (!dptr || !dxs || !dpart) return SPB_ERR_OOM;
   std::vector<Fr> xs(2 * count);
-  for (size_t q = 0; q < count; q++) { memcpy(&xs[2 * q], &points[q], 32); xs[2 * q + 1] = fp_pow_u64(xs[2 * q], T); }
+  for (size_t q = 0; q < count; q++) { xs[2 * q] = fr_load(&points[q]); xs[2 * q + 1] = fp_pow_u64(xs[2 * q], T); }
   SPB_CUDA(ctx, cudaMemcpyAsync((void*)dptr, d_polys, count * sizeof(void*), cudaMemcpyHostToDevice, d.stream));
   SPB_CUDA(ctx, cudaMemcpyAsync(dxs, xs.data(), xs.size() * sizeof(Fr), cudaMemcpyHostToDevice, d.stream));
-  eval_many_kernel<<<dim3(blocks, (unsigned)count), 256, 0, d.stream>>>(dptr, dxs, n, T, dpart);
-  SPB_CUDA(ctx, cudaGetLastError());
-  ctx->n_kernel_launches++;
+  SPB_TRY(launch(ctx, d.stream, dim3(blocks, (unsigned)count), 256, 0, eval_many_kernel, dptr, dxs, n, T, dpart));
   std::vector<Fr> part(count * blocks);
   SPB_CUDA(ctx, cudaMemcpyAsync(part.data(), dpart, part.size() * sizeof(Fr), cudaMemcpyDeviceToHost, d.stream));
   SPB_CUDA(ctx, cudaStreamSynchronize(d.stream));
@@ -553,11 +489,8 @@ int spb_eval_polynomial(spb_ctx* ctx, const spb_fr* poly, size_t n, const spb_fr
   Fr acc = fp_zero<FrParams>();
   if (n) {
     SPB_ENTER(ctx);
-    Fr* dp = (Fr*)slot(ctx, d, "poly_a", n * 32);
-    if (!dp) return SPB_ERR_OOM;
-    Fr x; memcpy(&x, point, 32);
-    SPB_CUDA(ctx, cudaMemcpyAsync(dp, poly, n * 32, cudaMemcpyHostToDevice, d.stream));
-    SPB_TRY(dev_eval_polynomial(ctx, d, dp, n, x, &acc));
+    SPB_TRY(run_staged(ctx, d, {{"poly_a", n * 32, poly, nullptr}},
+                       [&](void* const* p) { return dev_eval_polynomial(ctx, d, (const Fr*)p[0], n, fr_load(point), &acc); }));
   }
   memcpy(out, &acc, 32);
   return 0;
@@ -568,9 +501,7 @@ int spb_fr_random_chacha_dev(spb_ctx* ctx, const uint8_t seed[32], uint64_t firs
   if (!n) return 0;
   SPB_ENTER(ctx);
   ChaChaKey key; memcpy(key.w, seed, 32);
-  fr_random_chacha_kernel<<<nblk(n, 256), 256, 0, d.stream>>>(key, first, n, (Fr*)d_out);
-  SPB_CUDA(ctx, cudaGetLastError());
-  ctx->n_kernel_launches++;
+  SPB_TRY(launch(ctx, d.stream, nblk(n, 256), 256, 0, fr_random_chacha_kernel, key, first, n, (Fr*)d_out));
   SPB_CUDA(ctx, cudaStreamSynchronize(d.stream));
   return 0;
 }

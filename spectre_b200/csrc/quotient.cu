@@ -182,12 +182,11 @@ bool schedule_program(const uint32_t* words, size_t nwords, uint32_t ncalc, std:
 
 extern "C" {
 
-#define SPB_ENTER0(ctx)                         \
-  std::lock_guard<std::mutex> lk((ctx)->mu);    \
-  DeviceState& d0 = (ctx)->dev[0];              \
-  SPB_CUDA(ctx, cudaSetDevice(d0.device));      \
-  SPB_CUDA(ctx, cudaEventRecord(d0.ev0, d0.stream));  \
-  if ((ctx)->dev.size() > 1) SPB_CUDA(ctx, cudaEventRecord(d0.dep_ev, d0.stream));
+// SPB_ENTER, then start the pass clock and mark the point the other devices' shards wait for (shard_begin)
+#define SPB_ENTER0(ctx)                                  \
+  SPB_ENTER(ctx);                                        \
+  SPB_CUDA(ctx, cudaEventRecord(d.ev0, d.stream));       \
+  if ((ctx)->dev.size() > 1) SPB_CUDA(ctx, cudaEventRecord(d.dep_ev, d.stream));
 
 int spb_graph_evaluate_dev(spb_ctx* ctx, const spb_graph* g, const spb_fr* const* d_fixed, uint32_t n_fixed, const spb_fr* const* d_advice, uint32_t n_advice,
                            const spb_fr* const* d_instance, uint32_t n_instance, const spb_fr* challenges, uint32_t n_challenges, const spb_fr* beta,
@@ -207,34 +206,32 @@ int spb_graph_evaluate_dev(spb_ctx* ctx, const spb_graph* g, const spb_fr* const
   }
   SPB_ENTER0(ctx);
   std::vector<Fr> sc(4 + n_challenges);
-  memcpy(&sc[0], beta, 32); memcpy(&sc[1], gamma, 32); memcpy(&sc[2], theta, 32); memcpy(&sc[3], y, 32);
+  sc[0] = fr_load(beta); sc[1] = fr_load(gamma); sc[2] = fr_load(theta); sc[3] = fr_load(y);
   if (n_challenges) memcpy(&sc[4], challenges, (size_t)n_challenges * 32);
   const std::vector<RowRange> shards = row_ranges(ctx, size);
   for (auto& sh : shards) {
-    DeviceState& d = ctx->dev[sh.dev_index];
+    DeviceState& dv = ctx->dev[sh.dev_index];
     SPB_TRY(shard_begin(ctx, sh));
-    const uint32_t threads = 256, blocks = (uint32_t)d.sm_count * 2;   // grid-stride: 2 x 256 threads per SM
+    const uint32_t threads = 256, blocks = (uint32_t)dv.sm_count * 2;   // grid-stride: 2 x 256 threads per SM
     const uint64_t nslots = (uint64_t)threads * blocks;
     GraphArgs a; memset(&a, 0, sizeof a);
-    uint32_t* dprog = (uint32_t*)slot(ctx, d, "q_prog", (prog_n ? prog_n : 1) * 4);
-    Fr* dconst = (Fr*)slot(ctx, d, "q_const", (g->num_constants ? g->num_constants : 1) * sizeof(Fr));
-    int32_t* drot = (int32_t*)slot(ctx, d, "q_rot", (g->num_rotations ? g->num_rotations : 1) * 4);
-    Fr* dscal = (Fr*)slot(ctx, d, "q_scalars", (4 + (size_t)n_challenges) * sizeof(Fr));
-    Fr* scratch = (Fr*)slot(ctx, d, "q_scratch", (n_inter ? n_inter : 1) * nslots * sizeof(Fr));
+    uint32_t* dprog = (uint32_t*)slot(ctx, dv, "q_prog", (prog_n ? prog_n : 1) * 4);
+    Fr* dconst = (Fr*)slot(ctx, dv, "q_const", (g->num_constants ? g->num_constants : 1) * sizeof(Fr));
+    int32_t* drot = (int32_t*)slot(ctx, dv, "q_rot", (g->num_rotations ? g->num_rotations : 1) * 4);
+    Fr* dscal = (Fr*)slot(ctx, dv, "q_scalars", (4 + (size_t)n_challenges) * sizeof(Fr));
+    Fr* scratch = (Fr*)slot(ctx, dv, "q_scratch", (n_inter ? n_inter : 1) * nslots * sizeof(Fr));
     if (!dprog || !dconst || !drot || !dscal || !scratch) return SPB_ERR_OOM;
-    SPB_CUDA(ctx, cudaMemcpyAsync(dprog, prog, prog_n * 4, cudaMemcpyHostToDevice, d.stream));
-    if (g->num_constants) SPB_CUDA(ctx, cudaMemcpyAsync(dconst, g->constants, (size_t)g->num_constants * 32, cudaMemcpyHostToDevice, d.stream));
-    if (g->num_rotations) SPB_CUDA(ctx, cudaMemcpyAsync(drot, g->rotations, (size_t)g->num_rotations * 4, cudaMemcpyHostToDevice, d.stream));
-    SPB_CUDA(ctx, cudaMemcpyAsync(dscal, sc.data(), sc.size() * 32, cudaMemcpyHostToDevice, d.stream));
-    a.fixed = upload_ptrs(ctx, d, "q_fixed", d_fixed, n_fixed);
-    a.advice = upload_ptrs(ctx, d, "q_advice", d_advice, n_advice);
-    a.instance = upload_ptrs(ctx, d, "q_instance", d_instance, n_instance);
+    SPB_CUDA(ctx, cudaMemcpyAsync(dprog, prog, prog_n * 4, cudaMemcpyHostToDevice, dv.stream));
+    if (g->num_constants) SPB_CUDA(ctx, cudaMemcpyAsync(dconst, g->constants, (size_t)g->num_constants * 32, cudaMemcpyHostToDevice, dv.stream));
+    if (g->num_rotations) SPB_CUDA(ctx, cudaMemcpyAsync(drot, g->rotations, (size_t)g->num_rotations * 4, cudaMemcpyHostToDevice, dv.stream));
+    SPB_CUDA(ctx, cudaMemcpyAsync(dscal, sc.data(), sc.size() * 32, cudaMemcpyHostToDevice, dv.stream));
+    a.fixed = upload_ptrs(ctx, dv, "q_fixed", d_fixed, n_fixed);
+    a.advice = upload_ptrs(ctx, dv, "q_advice", d_advice, n_advice);
+    a.instance = upload_ptrs(ctx, dv, "q_instance", d_instance, n_instance);
     if (!a.fixed || !a.advice || !a.instance) return set_error(ctx, SPB_ERR_CUDA, "graph: pointer table upload failed");
     a.prog = dprog; a.ncalc = n_calc; a.constants = dconst; a.rotations = drot; a.scalars = dscal;
     a.values = (Fr*)d_values; a.scratch = scratch; a.size = size; a.rot_scale = rot_scale; a.row_lo = sh.lo; a.row_hi = sh.hi;
-    graph_evaluate_kernel<<<blocks, threads, 0, d.stream>>>(a);
-    SPB_CUDA(ctx, cudaGetLastError());
-    ctx->n_kernel_launches++;
+    SPB_TRY(launch(ctx, dv.stream, blocks, threads, 0, graph_evaluate_kernel, a));
   }
   return shards_finish(ctx, shards);  // synchronises: `sc` and the caller's arrays outlive the copies
 }
@@ -264,27 +261,24 @@ int spb_permutation_constraints_dev(spb_ctx* ctx, spb_fr* d_values, uint64_t siz
   a.values = (Fr*)d_values; a.size = size; a.rot_scale = rot_scale; a.last_rotation = last_rotation;
   a.n_sets = n_sets; a.chunk_len = chunk_len; a.n_cols = n_cols;
   a.l0 = (const Fr*)d_l0; a.l_last = (const Fr*)d_l_last; a.l_active = (const Fr*)d_l_active;
-  memcpy(&a.beta, beta, 32); memcpy(&a.gamma, gamma, 32); memcpy(&a.y, y, 32); memcpy(&a.extended_omega, extended_omega, 32);
-  Fr zeta; { constexpr uint32_t v[8] = SPB_FR_ZETA_MONT; for (int i = 0; i < 8; i++) zeta.l[i] = v[i]; }
-  { constexpr uint32_t v[8] = SPB_FR_DELTA_MONT; for (int i = 0; i < 8; i++) a.delta.l[i] = v[i]; }
-  a.delta_start = fp_mul(a.beta, zeta);
+  a.beta = fr_load(beta); a.gamma = fr_load(gamma); a.y = fr_load(y); a.extended_omega = fr_load(extended_omega);
+  a.delta = fr_delta();
+  a.delta_start = fp_mul(a.beta, fr_zeta());
   std::vector<Fr> pw(256);
   pw[0] = fp_one<FrParams>();
   for (int j = 1; j < 256; j++) pw[j] = fp_mul(pw[j - 1], a.extended_omega);
   const std::vector<RowRange> shards = row_ranges(ctx, size);
   for (auto& sh : shards) {
-    DeviceState& d = ctx->dev[sh.dev_index];
+    DeviceState& dv = ctx->dev[sh.dev_index];
     SPB_TRY(shard_begin(ctx, sh));
-    a.z = upload_ptrs(ctx, d, "q_z", d_z, n_sets);
-    a.col_values = upload_ptrs(ctx, d, "q_cols", d_col_values, n_cols);
-    a.sigma = upload_ptrs(ctx, d, "q_sigma", d_sigma, n_cols);
-    Fr* dpw = (Fr*)slot(ctx, d, "q_omega_pow", 256 * sizeof(Fr));
+    a.z = upload_ptrs(ctx, dv, "q_z", d_z, n_sets);
+    a.col_values = upload_ptrs(ctx, dv, "q_cols", d_col_values, n_cols);
+    a.sigma = upload_ptrs(ctx, dv, "q_sigma", d_sigma, n_cols);
+    Fr* dpw = (Fr*)slot(ctx, dv, "q_omega_pow", 256 * sizeof(Fr));
     if (!a.z || !a.col_values || !a.sigma || !dpw) return set_error(ctx, SPB_ERR_CUDA, "permutation: table upload failed");
-    SPB_CUDA(ctx, cudaMemcpyAsync(dpw, pw.data(), 256 * sizeof(Fr), cudaMemcpyHostToDevice, d.stream));
+    SPB_CUDA(ctx, cudaMemcpyAsync(dpw, pw.data(), 256 * sizeof(Fr), cudaMemcpyHostToDevice, dv.stream));
     a.omega_pow = dpw; a.row_lo = sh.lo; a.row_hi = sh.hi;
-    permutation_constraints_kernel<<<(unsigned)((sh.hi - sh.lo + 255) / 256), 256, 0, d.stream>>>(a);
-    SPB_CUDA(ctx, cudaGetLastError());
-    ctx->n_kernel_launches++;
+    SPB_TRY(launch(ctx, dv.stream, nblk(sh.hi - sh.lo, 256), 256, 0, permutation_constraints_kernel, a));
   }
   return shards_finish(ctx, shards);
 }
@@ -300,15 +294,12 @@ int spb_lookup_constraints_dev(spb_ctx* ctx, spb_fr* d_values, uint64_t size, in
   a.values = (Fr*)d_values; a.size = size; a.rot_scale = rot_scale;
   a.product = (const Fr*)d_product; a.permuted_input = (const Fr*)d_permuted_input; a.permuted_table = (const Fr*)d_permuted_table;
   a.table_value = (const Fr*)d_table_value; a.l0 = (const Fr*)d_l0; a.l_last = (const Fr*)d_l_last; a.l_active = (const Fr*)d_l_active;
-  memcpy(&a.beta, beta, 32); memcpy(&a.gamma, gamma, 32); memcpy(&a.y, y, 32);
+  a.beta = fr_load(beta); a.gamma = fr_load(gamma); a.y = fr_load(y);
   const std::vector<RowRange> shards = row_ranges(ctx, size);
   for (auto& sh : shards) {
-    DeviceState& d = ctx->dev[sh.dev_index];
     SPB_TRY(shard_begin(ctx, sh));
     a.row_lo = sh.lo; a.row_hi = sh.hi;
-    lookup_constraints_kernel<<<(unsigned)((sh.hi - sh.lo + 255) / 256), 256, 0, d.stream>>>(a);
-    SPB_CUDA(ctx, cudaGetLastError());
-    ctx->n_kernel_launches++;
+    SPB_TRY(launch(ctx, ctx->dev[sh.dev_index].stream, nblk(sh.hi - sh.lo, 256), 256, 0, lookup_constraints_kernel, a));
   }
   return shards_finish(ctx, shards);
 }
