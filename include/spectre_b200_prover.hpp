@@ -653,11 +653,19 @@ class Engine {
 
 // ---- keygen ---------------------------------------------------------------------------------------------------------------
 using Cell = std::pair<uint32_t, uint64_t>;                  // (index in cs.permutation, row)
+// Residency of a key's extended cosets (spectre_b200/plonk.py, COSETS_MODES). Resident: fixed, sigma and l0 / l_last / l_active
+// cosets stay in device memory with the key. OnDemand (a lean key): the key holds only its n-row data, with the three l
+// polynomials in coefficient form in `l_polys`, and create_proof rebuilds the cosets for each proof and frees them after the
+// quotient. The proof bytes are the same in both modes. CudaMemory keeps the freed cosets on its free lists for the next proof;
+// a process that holds several keys calls trim() after a proof to give them back to the device.
+enum class Cosets { Resident, OnDemand };
 struct ProvingKey {
   ConstraintSystem cs;                                      // held by value (expression nodes are shared_ptr): a cached key never dangles
   uint32_t k = 0; size_t n = 0; uint32_t blinding_factors = 0; size_t usable_rows = 0;
+  Cosets cosets = Cosets::Resident;
   std::vector<Buffer> fixed_values, fixed_polys, fixed_cosets, sigma_values, sigma_polys, sigma_cosets;
-  Buffer l0, l_last, l_active;
+  Buffer l0, l_last, l_active;                              // Resident only
+  std::vector<Buffer> l_polys;                              // OnDemand only: l0, l_last, l_active in coefficient form
   std::vector<Point> fixed_commitments, sigma_commitments;
   U256 vk_digest{};
 };
@@ -702,30 +710,31 @@ inline U256 default_vk_digest(const ProvingKey& pk) {
   return hostfield::reduce(FrP(), hostfield::from_be(h.data()));
 }
 
-// fixed_columns: host arrays of n Montgomery elements (Lagrange basis)
+// fixed_columns: host arrays of n Montgomery elements (Lagrange basis). cosets = OnDemand makes a lean key: no coset is computed.
 inline ProvingKey keygen(Engine& E, const ConstraintSystem& cs, const std::vector<const Fr*>& fixed_columns, const std::vector<std::pair<Cell, Cell>>& copies,
-                         const U256* vk_digest = nullptr) {
+                         const U256* vk_digest = nullptr, Cosets cosets = Cosets::Resident) {
   ProvingKey pk;
-  pk.cs = cs; pk.k = E.k; pk.n = E.n;
+  pk.cs = cs; pk.k = E.k; pk.n = E.n; pk.cosets = cosets;
   pk.blinding_factors = cs.blinding_factors(); pk.usable_rows = E.n - (pk.blinding_factors + 1);
   for (auto* c : fixed_columns) pk.fixed_values.push_back(E.upload(c, E.n));
   pk.sigma_values = build_sigma(E, cs, copies);
   if (!pk.fixed_values.empty()) pk.fixed_commitments = E.commit(SPB_BASIS_G_LAGRANGE, ptrs(pk.fixed_values), E.n);
   if (!pk.sigma_values.empty()) pk.sigma_commitments = E.commit(SPB_BASIS_G_LAGRANGE, ptrs(pk.sigma_values), E.n);
+  const bool resident = cosets == Cosets::Resident;
   auto poly_and_coset = [&](const Buffer& values, std::vector<Buffer>* polys, std::vector<Buffer>* cosets) {
     Buffer p = E.clone(values); E.lagrange_to_coeff(p);
-    Buffer c = E.coeff_to_extended(p);
+    if (resident) cosets->push_back(E.coeff_to_extended(p));
     if (polys) polys->push_back(std::move(p));
-    cosets->push_back(std::move(c));
   };
   for (auto& v : pk.fixed_values) poly_and_coset(v, &pk.fixed_polys, &pk.fixed_cosets);
   for (auto& v : pk.sigma_values) poly_and_coset(v, &pk.sigma_polys, &pk.sigma_cosets);
   const Fr one = fr_mont(u256(1));
   std::vector<Buffer> ls;
-  { Buffer l0 = E.alloc(E.n); E.write_rows(l0, 0, &one, 1); poly_and_coset(l0, nullptr, &ls); }
-  { Buffer ll = E.alloc(E.n); E.write_rows(ll, pk.usable_rows, &one, 1); poly_and_coset(ll, nullptr, &ls); }
-  { Buffer la = E.alloc(E.n); std::vector<Fr> ones(pk.usable_rows, one); E.write_rows(la, 0, ones.data(), ones.size()); poly_and_coset(la, nullptr, &ls); }
-  pk.l0 = std::move(ls[0]); pk.l_last = std::move(ls[1]); pk.l_active = std::move(ls[2]);
+  std::vector<Buffer>* l_polys = resident ? nullptr : &pk.l_polys;
+  { Buffer l0 = E.alloc(E.n); E.write_rows(l0, 0, &one, 1); poly_and_coset(l0, l_polys, &ls); }
+  { Buffer ll = E.alloc(E.n); E.write_rows(ll, pk.usable_rows, &one, 1); poly_and_coset(ll, l_polys, &ls); }
+  { Buffer la = E.alloc(E.n); std::vector<Fr> ones(pk.usable_rows, one); E.write_rows(la, 0, ones.data(), ones.size()); poly_and_coset(la, l_polys, &ls); }
+  if (resident) { pk.l0 = std::move(ls[0]); pk.l_last = std::move(ls[1]); pk.l_active = std::move(ls[2]); }
   pk.vk_digest = vk_digest ? *vk_digest : default_vk_digest(pk);
   return pk;
 }
@@ -876,26 +885,40 @@ inline std::vector<uint8_t> create_proof(Engine& E, const ProvingKey& pk, const 
   Buffer h_coeff;
   const uint32_t pieces_n = (uint32_t)cs.degree() - 1;
   {
+    // a lean key's cosets are rebuilt here and released with the advice cosets, before divide_by_vanishing
+    const bool lean = pk.cosets == Cosets::OnDemand;
+    std::vector<Buffer> key_fixed, key_sigma, key_l;
+    if (lean) {
+      for (auto& p : pk.fixed_polys) key_fixed.push_back(E.coeff_to_extended(p));
+      for (auto& p : pk.sigma_polys) key_sigma.push_back(E.coeff_to_extended(p));
+      for (auto& p : pk.l_polys) key_l.push_back(E.coeff_to_extended(p));
+    }
+    const std::vector<Buffer>& fixed_cosets = lean ? key_fixed : pk.fixed_cosets;
+    const std::vector<Buffer>& sigma_cosets = lean ? key_sigma : pk.sigma_cosets;
+    const Buffer& l0 = lean ? key_l[0] : pk.l0;
+    const Buffer& l_last = lean ? key_l[1] : pk.l_last;
+    const Buffer& l_active = lean ? key_l[2] : pk.l_active;
     std::vector<Buffer> advice_cosets, inst_cosets;
     for (auto& p : advice_polys) advice_cosets.push_back(E.coeff_to_extended(p));
     for (auto& p : inst_polys) inst_cosets.push_back(E.coeff_to_extended(p));
     Buffer values = E.alloc(ext_n);
-    if (!cs.gates.empty()) E.graph_evaluate(cs.gates_program(), ptrs(pk.fixed_cosets), ptrs(advice_cosets), ptrs(inst_cosets), beta, gamma, theta, y, values, ext_n, rot_scale);
+    if (!cs.gates.empty()) E.graph_evaluate(cs.gates_program(), ptrs(fixed_cosets), ptrs(advice_cosets), ptrs(inst_cosets), beta, gamma, theta, y, values, ext_n, rot_scale);
     if (!perm_polys.empty()) {
       std::vector<Buffer> z_cosets;
       for (auto& p : perm_polys) z_cosets.push_back(E.coeff_to_extended(p));
       std::vector<const Fr*> cosets;
-      for (auto& pc : cs.permutation) cosets.push_back(column(pc, pk.fixed_cosets, advice_cosets, inst_cosets));
+      for (auto& pc : cs.permutation) cosets.push_back(column(pc, fixed_cosets, advice_cosets, inst_cosets));
       U256 ew = root_of_unity(); for (uint32_t i = E.extended_k; i < 28; i++) ew = mulmod(ew, ew);
-      E.permutation_constraints(values, ext_n, rot_scale, -(int32_t)(bf + 1), chunk, ptrs(z_cosets), cosets, ptrs(pk.sigma_cosets), pk.l0, pk.l_last, pk.l_active, beta, gamma, y, fr_mont(ew));
+      E.permutation_constraints(values, ext_n, rot_scale, -(int32_t)(bf + 1), chunk, ptrs(z_cosets), cosets, ptrs(sigma_cosets), l0, l_last, l_active, beta, gamma, y, fr_mont(ew));
     }
     for (size_t li = 0; li < lookups.size(); li++) {
       L& l = lookups[li];
       Buffer table_value = E.alloc(ext_n);
-      E.graph_evaluate(cs.lookup_value_program(li), ptrs(pk.fixed_cosets), ptrs(advice_cosets), ptrs(inst_cosets), beta, gamma, theta, zero4, table_value, ext_n, rot_scale);
+      E.graph_evaluate(cs.lookup_value_program(li), ptrs(fixed_cosets), ptrs(advice_cosets), ptrs(inst_cosets), beta, gamma, theta, zero4, table_value, ext_n, rot_scale);
       Buffer pc = E.coeff_to_extended(l.product), ic = E.coeff_to_extended(l.permuted_input_poly), tc = E.coeff_to_extended(l.permuted_table_poly);
-      E.lookup_constraints(values, ext_n, rot_scale, pc, ic, tc, table_value, pk.l0, pk.l_last, pk.l_active, beta, gamma, y);
+      E.lookup_constraints(values, ext_n, rot_scale, pc, ic, tc, table_value, l0, l_last, l_active, beta, gamma, y);
     }
+    key_fixed.clear(); key_sigma.clear(); key_l.clear(); advice_cosets.clear(); inst_cosets.clear();
     E.divide_by_vanishing(values);
     h_coeff = E.extended_to_coeff(values, n * pieces_n);
   }

@@ -116,3 +116,6 @@ impl FlatGraph {
 // -- the same sequence as spectre_b200/plonk.py::create_proof stage 7 and include/spectre_b200_prover.hpp, whose proofs
 // the reference's verifier contracts accept (DESIGN.md section 2). On a context with several devices each of these
 // passes is split into row ranges across the devices by the library; nothing changes on this side.
+// With a lean proving key (INTEGRATION.md section 4, "Key residency") fixed_cosets, sigma_cosets and l0 / l_last / l_active
+// are not held by the key: they are rebuilt from the key's coefficient forms by one spb_coeff_to_extended_batch_dev call
+// just before this sequence and freed after it, before divide_by_vanishing. The sequence itself does not change.

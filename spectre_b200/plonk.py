@@ -374,8 +374,47 @@ def coeff_to_extended_many(E, bufs):
 
 
 # ---- keygen -------------------------------------------------------------------------------------------------------
+# Residency of a proving key's extended cosets (fixed, sigma, l0 / l_last / l_active: 2^extended_k rows each, about three
+# quarters of a key's bytes). "resident" keeps them in device memory for the life of the key. "on_demand" (a lean key) keeps
+# only the n-row data -- fixed / sigma values and polys, and the three l polynomials in coefficient form -- and create_proof
+# rebuilds the cosets before the quotient and frees them after it. A rebuilt coset is the same coset, so the proof bytes are
+# the same in both modes; a lean key costs one coset NTT per fixed / sigma / l column per proof.
+COSETS_MODES = ("resident", "on_demand")
+
+
 class ProvingKey:
-    pass
+    """A lean key (cosets="on_demand") has fixed_cosets = sigma_cosets = l0 = l_last = l_active = None and holds `l_polys`
+    = [l0, l_last, l_active] in coefficient form instead (None in a resident key)."""
+
+    @property
+    def lean(self):
+        return self.fixed_cosets is None
+
+
+def key_device_bytes(cs, k, extended_k, cosets="resident"):
+    """Device bytes a proving key of this shape holds (DESIGN.md section 3), with C = num_fixed + len(permutation) columns:
+    32 * (2 C 2^k + (C + 3) 2^extended_k) resident, 32 * (2 C + 3) 2^k lean."""
+    _check_cosets_mode(cosets)
+    cols = cs.num_fixed + len(cs.permutation)
+    if cosets == "resident":
+        return 32 * ((2 * cols << k) + ((cols + 3) << extended_k))
+    return 32 * ((2 * cols + 3) << k)
+
+
+def _check_cosets_mode(cosets):
+    if cosets not in COSETS_MODES:
+        raise ValueError("cosets must be one of %s, not %r" % (", ".join(COSETS_MODES), cosets))
+
+
+def l_polys(E, n, usable_rows):
+    """[l0, l_last, l_active] in coefficient form: l_active = 1 - l_last - l_blind is one on the rows [0, usable_rows)"""
+    one = fr_mont(1).reshape(1, 4)
+    l0 = E.alloc(n); E.write_rows(l0, 0, one)
+    l_last = E.alloc(n); E.write_rows(l_last, usable_rows, one)
+    l_active = E.alloc(n); E.write_rows(l_active, 0, np.broadcast_to(one, (usable_rows, 4)))
+    ls = [l0, l_last, l_active]
+    lagrange_to_coeff_many(E, ls)
+    return ls
 
 
 def build_sigma(E, cs, k, copies):
@@ -414,9 +453,11 @@ def build_sigma(E, cs, k, copies):
     return sigma
 
 
-def keygen(E, cs, k, fixed_columns, copies, vk_digest=None):
+def keygen(E, cs, k, fixed_columns, copies, vk_digest=None, cosets="resident"):
     """keygen_vk + keygen_pk: fixed and sigma commitments, their coefficient forms and extended cosets, l0 / l_last /
-    l_active cosets -- all left resident on the device. fixed_columns: list of (n, 4) Montgomery arrays (Lagrange)."""
+    l_active cosets -- all left resident on the device. fixed_columns: list of (n, 4) Montgomery arrays (Lagrange).
+    cosets="on_demand" makes a lean key: no coset is ever computed, create_proof rebuilds them for each proof."""
+    _check_cosets_mode(cosets)
     n = 1 << k
     pk = ProvingKey()
     pk.cs, pk.k, pk.n = cs, k, n
@@ -428,19 +469,20 @@ def keygen(E, cs, k, fixed_columns, copies, vk_digest=None):
     pk.fixed_commitments = E.commit(G_LAG, pk.fixed_values, n) if pk.fixed_values else []
     pk.sigma_commitments = E.commit(G_LAG, pk.sigma_values, n) if pk.sigma_values else []
 
-    def polys_and_cosets(values):
+    def polys(values):
         ps = [E.clone(v) for v in values]
         lagrange_to_coeff_many(E, ps)
-        return ps, coeff_to_extended_many(E, ps)
-    pk.fixed_polys, pk.fixed_cosets = polys_and_cosets(pk.fixed_values)
-    pk.sigma_polys, pk.sigma_cosets = polys_and_cosets(pk.sigma_values)
-    one = fr_mont(1).reshape(1, 4)
-    l0 = E.alloc(n); E.write_rows(l0, 0, one)
-    l_last = E.alloc(n); E.write_rows(l_last, pk.usable_rows, one)
-    # l_active = 1 - l_last - l_blind on the evaluation rows: ones on rows [0, usable_rows)
-    l_active = E.alloc(n)
-    E.write_rows(l_active, 0, np.broadcast_to(one, (pk.usable_rows, 4)))
-    pk.l0, pk.l_last, pk.l_active = polys_and_cosets([l0, l_last, l_active])[1]
+        return ps
+    pk.fixed_polys, pk.sigma_polys = polys(pk.fixed_values), polys(pk.sigma_values)
+    ls = l_polys(E, n, pk.usable_rows)
+    if cosets == "resident":
+        pk.fixed_cosets = coeff_to_extended_many(E, pk.fixed_polys)
+        pk.sigma_cosets = coeff_to_extended_many(E, pk.sigma_polys)
+        pk.l0, pk.l_last, pk.l_active = coeff_to_extended_many(E, ls)
+        pk.l_polys = None
+    else:
+        pk.fixed_cosets = pk.sigma_cosets = pk.l0 = pk.l_last = pk.l_active = None
+        pk.l_polys = ls
     pk.vk_digest = vk_digest if vk_digest is not None else default_vk_digest(pk)
     return pk
 
@@ -482,7 +524,8 @@ def _point_from(raw):
 
 def write_pk(E, pk, path):
     """ProvingKey::write(writer, SerdeFormat::RawBytesUnchecked): header and commitments from the host, every polynomial
-    streamed from device memory by the engine."""
+    streamed from device memory by the engine. A lean key writes the same bytes: each coset is rebuilt into one temporary
+    buffer, appended and freed before the next."""
     with open(path, "wb") as f:
         f.write(pk.k.to_bytes(4, "big") + len(pk.fixed_commitments).to_bytes(4, "big"))
         for pt in pk.fixed_commitments + pk.sigma_commitments:
@@ -493,20 +536,30 @@ def write_pk(E, pk, path):
             f.write(rows.to_bytes(4, "big"))
         E.append_to_file(path, b, rows)
 
-    def polys(bufs, rows):
+    def polys(bufs, rows, count):
         with open(path, "ab") as f:
-            f.write(len(bufs).to_bytes(4, "big"))
+            f.write(count.to_bytes(4, "big"))
         for b in bufs:
             poly(b, rows)
+            del b                                            # a rebuilt coset is freed before the next one is built
+
+    def cosets(resident, coeffs):
+        return resident if resident is not None else (E.coeff_to_extended(p) for p in coeffs)
     ext = 1 << E.extended_k
-    for b in (pk.l0, pk.l_last, pk.l_active):
+    for b in cosets(None if pk.lean else [pk.l0, pk.l_last, pk.l_active], pk.l_polys):
         poly(b, ext)
-    polys(pk.fixed_values, pk.n); polys(pk.fixed_polys, pk.n); polys(pk.fixed_cosets, ext)
-    polys(pk.sigma_values, pk.n); polys(pk.sigma_polys, pk.n); polys(pk.sigma_cosets, ext)
+        del b
+    nf, m = len(pk.fixed_polys), len(pk.sigma_polys)
+    polys(pk.fixed_values, pk.n, nf); polys(pk.fixed_polys, pk.n, nf); polys(cosets(pk.fixed_cosets, pk.fixed_polys), ext, nf)
+    polys(pk.sigma_values, pk.n, m); polys(pk.sigma_polys, pk.n, m); polys(cosets(pk.sigma_cosets, pk.sigma_polys), ext, m)
 
 
-def read_pk(E, cs, path, vk_digest=None):
-    """ProvingKey::read: the inverse of write_pk; `cs` plays the role of the concrete circuit's configure()."""
+def read_pk(E, cs, path, vk_digest=None, cosets="resident"):
+    """ProvingKey::read: the inverse of write_pk; `cs` plays the role of the concrete circuit's configure().
+    cosets="on_demand" reads a lean key from the same file: the coset sections are skipped, never read, and the three l
+    polynomials are rebuilt from their definition."""
+    _check_cosets_mode(cosets)
+    lean = cosets == "on_demand"
     pk = ProvingKey()
     with open(path, "rb") as f:
         head = f.read(8)
@@ -527,23 +580,25 @@ def read_pk(E, cs, path, vk_digest=None):
         pos[0] += 4
         return v
 
-    def poly(rows):
+    def poly(rows, skip=False):
         if u32() != rows:
             raise ValueError("read_pk: polynomial length mismatch in %s" % path)
-        b = E.read_from_file(path, pos[0], rows)
+        b = None if skip else E.read_from_file(path, pos[0], rows)
         pos[0] += rows * 32
         return b
 
-    def polys(count, rows):
+    def polys(count, rows, skip=False):
         if u32() != count:
             raise ValueError("read_pk: slice length mismatch in %s" % path)
-        return [poly(rows) for _ in range(count)]
-    pk.l0, pk.l_last, pk.l_active = poly(ext), poly(ext), poly(ext)
-    pk.fixed_values, pk.fixed_polys, pk.fixed_cosets = polys(n_fixed, n), polys(n_fixed, n), polys(n_fixed, ext)
+        bufs = [poly(rows, skip) for _ in range(count)]
+        return None if skip else bufs
+    pk.l0, pk.l_last, pk.l_active = poly(ext, lean), poly(ext, lean), poly(ext, lean)
+    pk.fixed_values, pk.fixed_polys, pk.fixed_cosets = polys(n_fixed, n), polys(n_fixed, n), polys(n_fixed, ext, lean)
     m = len(cs.permutation)
-    pk.sigma_values, pk.sigma_polys, pk.sigma_cosets = polys(m, n), polys(m, n), polys(m, ext)
+    pk.sigma_values, pk.sigma_polys, pk.sigma_cosets = polys(m, n), polys(m, n), polys(m, ext, lean)
     if pos[0] != size:
         raise ValueError("read_pk: %d trailing bytes in %s" % (size - pos[0], path))
+    pk.l_polys = l_polys(E, n, pk.usable_rows) if lean else None
     pk.vk_digest = vk_digest if vk_digest is not None else default_vk_digest(pk)
     return pk
 
@@ -688,26 +743,35 @@ def create_proof(E, pk, instances, advice_columns, rng, transcript, timings=None
     y = fr_mont(transcript.squeeze_challenge())
 
     # 7. quotient: extended cosets, evaluate_h, divide by the vanishing polynomial, split, commit
+    # a lean key's cosets are rebuilt here and freed with the advice cosets, before divide_by_vanishing
+    if pk.lean:
+        nf, ns = len(pk.fixed_polys), len(pk.sigma_polys)
+        key = coeff_to_extended_many(E, pk.fixed_polys + pk.sigma_polys + pk.l_polys)
+        fixed_cosets, sigma_cosets, (l0, l_last, l_active) = key[:nf], key[nf:nf + ns], key[nf + ns:]
+        del key
+        lap("key_cosets")
+    else:
+        fixed_cosets, sigma_cosets, l0, l_last, l_active = pk.fixed_cosets, pk.sigma_cosets, pk.l0, pk.l_last, pk.l_active
     both = coeff_to_extended_many(E, advice_polys + inst_polys)
     advice_cosets, inst_cosets = both[:len(advice_polys)], both[len(advice_polys):]
     del both
     lap("coeff_to_extended")
     values = E.alloc(ext_n)
     if cs.gates:
-        E.graph_evaluate(cs.gates_program(), pk.fixed_cosets, advice_cosets, inst_cosets, beta, gamma, theta, y, values, ext_n, rot_scale)
+        E.graph_evaluate(cs.gates_program(), fixed_cosets, advice_cosets, inst_cosets, beta, gamma, theta, y, values, ext_n, rot_scale)
     if perm_polys:
         z_cosets = coeff_to_extended_many(E, perm_polys)
-        cosets = [{"fixed": pk.fixed_cosets, "advice": advice_cosets, "instance": inst_cosets}[kind][c] for kind, c in cs.permutation]
+        cosets = [{"fixed": fixed_cosets, "advice": advice_cosets, "instance": inst_cosets}[kind][c] for kind, c in cs.permutation]
         ext_omega = fr_mont(pow(ROOT_OF_UNITY, 1 << (28 - E.extended_k), R_MOD))
-        E.permutation_constraints(values, ext_n, rot_scale, -(bf + 1), chunk, z_cosets, cosets, pk.sigma_cosets, pk.l0, pk.l_last, pk.l_active, beta, gamma, y, ext_omega)
-        del z_cosets
+        E.permutation_constraints(values, ext_n, rot_scale, -(bf + 1), chunk, z_cosets, cosets, sigma_cosets, l0, l_last, l_active, beta, gamma, y, ext_omega)
+        del z_cosets, cosets
     for li, L in enumerate(lookups):
         table_value = E.alloc(ext_n)
-        E.graph_evaluate(cs.lookup_value_program(li), pk.fixed_cosets, advice_cosets, inst_cosets, beta, gamma, theta, zero4, table_value, ext_n, rot_scale)
+        E.graph_evaluate(cs.lookup_value_program(li), fixed_cosets, advice_cosets, inst_cosets, beta, gamma, theta, zero4, table_value, ext_n, rot_scale)
         pc, ic, tc = coeff_to_extended_many(E, [L.product_poly, L.permuted_input_poly, L.permuted_table_poly])
-        E.lookup_constraints(values, ext_n, rot_scale, pc, ic, tc, table_value, pk.l0, pk.l_last, pk.l_active, beta, gamma, y)
+        E.lookup_constraints(values, ext_n, rot_scale, pc, ic, tc, table_value, l0, l_last, l_active, beta, gamma, y)
         del table_value, pc, ic, tc
-    del advice_cosets, inst_cosets
+    del advice_cosets, inst_cosets, fixed_cosets, sigma_cosets, l0, l_last, l_active
     lap("evaluate_h")
     E.divide_by_vanishing(values)
     pieces_n = cs.degree() - 1

@@ -10,15 +10,16 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def build_main_against_the_real_library(out_dir=None):
-    """g++ tests/cpp/prover_main.cpp -DSPB_PROVER_WITH_CUDART against libspectre_b200.so + cudart -> <out_dir>/prover_main_cuda
-    (default out_dir: a new temporary directory -- the checkout may be read-only)"""
+def build_main_against_the_real_library(out_dir=None, main="prover_main"):
+    """g++ tests/cpp/<main>.cpp -DSPB_PROVER_WITH_CUDART against libspectre_b200.so + cudart -> <out_dir>/<main>_cuda
+    (default out_dir: a new temporary directory -- the checkout may be read-only). main="prover_main_lean" proves with a
+    lean key (cosets rebuilt per proof)."""
     from spectre_b200 import build
     lib = build.build()
     libdir = os.path.dirname(lib)
-    exe = os.path.join(out_dir or tempfile.mkdtemp(prefix="spb_prover_main_"), "prover_main_cuda")
-    src = os.path.join(ROOT, "tests", "cpp", "prover_main.cpp")
-    hdrs = [os.path.join(ROOT, "include", h) for h in ("spectre_b200.h", "spectre_b200_prover.hpp")]
+    exe = os.path.join(out_dir or tempfile.mkdtemp(prefix="spb_prover_main_"), main + "_cuda")
+    src = os.path.join(ROOT, "tests", "cpp", main + ".cpp")
+    hdrs = [os.path.join(ROOT, "include", h) for h in ("spectre_b200.h", "spectre_b200_prover.hpp")] + [os.path.join(ROOT, "tests", "cpp", "prover_main.cpp")]
     if os.path.exists(exe) and os.path.getmtime(exe) >= max(os.path.getmtime(p) for p in [src, lib] + hdrs):
         return exe
     cuda = os.environ.get("CUDA_HOME", "/usr/local/cuda")
