@@ -199,6 +199,14 @@ int spb_divide_by_vanishing_dev(spb_ctx* ctx, const spb_domain* d, spb_fr* d_a);
  * first device through NVLink peer access (SURVEY.md 8e: NTTs sharded by polynomial). HOST arrays of device pointers. */
 int spb_lagrange_to_coeff_batch_dev(spb_ctx* ctx, const spb_domain* d, spb_fr* const* d_a, size_t count);
 int spb_coeff_to_extended_batch_dev(spb_ctx* ctx, const spb_domain* d, const spb_fr* const* d_in, spb_fr* const* d_out, size_t count);
+/* Coset part `part` of coeff_to_extended, for evaluating the quotient one n-row part at a time. With R = 2^(extended_k - k),
+ * d_out[i][m] = coeff_to_extended(d_in[i])[part + R m] for m < 2^k: the values at g omega^m, g = zeta extended_omega^part,
+ * computed as one 2^k-point transform of the coefficients pre-scaled by g^a. Out of place (d_in is never written); spread over
+ * the devices like spb_coeff_to_extended_batch_dev. part >= R: SPB_ERR_ARG. HOST arrays of device pointers. */
+int spb_coeff_to_extended_part_batch_dev(spb_ctx* ctx, const spb_domain* d, uint32_t part, const spb_fr* const* d_in, spb_fr* const* d_out, size_t count);
+/* d_extended[part + R m] = d_part[m] for m < 2^k: a coset part back into its rows of a 2^extended_k buffer. Rows are sharded
+ * over the context's devices like the quotient passes. part >= R: SPB_ERR_ARG. */
+int spb_extended_part_scatter_dev(spb_ctx* ctx, const spb_domain* d, uint32_t part, const spb_fr* d_part, spb_fr* d_extended);
 
 /* ---- batch polynomial arithmetic ([UPSTREAM] halo2_proofs/src/arithmetic.rs, ff::BatchInvert) ---------- */
 /* Zero-length inputs: with n = 0, spb_vec_{mul,axpy,scale}, spb_grand_product, spb_batch_invert (host and _dev forms),
@@ -269,6 +277,13 @@ int spb_permutation_constraints_dev(spb_ctx* ctx, spb_fr* d_values, uint64_t siz
                                     const spb_fr* const* d_z, uint32_t n_cols, const spb_fr* const* d_col_values, const spb_fr* const* d_sigma,
                                     const spb_fr* d_l0, const spb_fr* d_l_last, const spb_fr* d_l_active, const spb_fr* beta, const spb_fr* gamma,
                                     const spb_fr* y, const spb_fr* extended_omega);
+/* the same terms with X = coset_generator * omega^idx at row idx: over coset part j of the extended coset (size = 2^k,
+ * rot_scale = 1, every input a part from spb_coeff_to_extended_part_batch_dev) coset_generator = zeta extended_omega^j and
+ * omega = the 2^k-th root. (zeta, extended_omega) gives spb_permutation_constraints_dev. */
+int spb_permutation_constraints_coset_dev(spb_ctx* ctx, spb_fr* d_values, uint64_t size, int32_t rot_scale, int32_t last_rotation, uint32_t n_sets,
+                                          uint32_t chunk_len, const spb_fr* const* d_z, uint32_t n_cols, const spb_fr* const* d_col_values,
+                                          const spb_fr* const* d_sigma, const spb_fr* d_l0, const spb_fr* d_l_last, const spb_fr* d_l_active,
+                                          const spb_fr* beta, const spb_fr* gamma, const spb_fr* y, const spb_fr* coset_generator, const spb_fr* omega);
 /* the five lookup-argument terms of one lookup; d_table_value[idx] = (compressed input + beta)(compressed table + gamma) */
 int spb_lookup_constraints_dev(spb_ctx* ctx, spb_fr* d_values, uint64_t size, int32_t rot_scale, const spb_fr* d_product, const spb_fr* d_permuted_input,
                                const spb_fr* d_permuted_table, const spb_fr* d_table_value, const spb_fr* d_l0, const spb_fr* d_l_last,

@@ -29,6 +29,13 @@
 
 #include "spectre_b200.h"
 
+// The entry points only a per-part key's proof calls are referenced weakly: a program built on this header and linked against
+// a build of the C ABI without them still proves with resident and lean keys, and a per-part proof there fails with an error
+// naming what is missing (Engine::has_per_part) instead of the whole program failing to link.
+#pragma weak spb_coeff_to_extended_part_batch_dev
+#pragma weak spb_extended_part_scatter_dev
+#pragma weak spb_permutation_constraints_coset_dev
+
 namespace halo2 {
 namespace hostfield {
 
@@ -305,6 +312,8 @@ inline U256 mulmod(const U256& a, const U256& b) {   // canonical * canonical ->
 inline U256 powmod(const U256& a, uint64_t e) { return hostfield::from_mont(FrP(), hostfield::pow_u64(FrP(), hostfield::to_mont(FrP(), a), e)); }
 inline U256 root_of_unity() { return hostfield::from_mont(FrP(), {0x9632c7c5b639feb8ull, 0x985ce3400d0ff299ull, 0xb2dd880001b0ecd8ull, 0x1d69070d6d98ce29ull}); }
 inline U256 delta() { return hostfield::from_mont(FrP(), {0x9a0c322befd78855ull, 0x46e82d14249b563cull, 0x5983a663e0b0b7a7ull, 0x22ab452baaa111adull}); }
+// the extended coset's shift (EvaluationDomain g_coset): a cube root of unity
+inline U256 zeta() { return hostfield::from_mont(FrP(), {0x0363f29955fcd653ull, 0x73e7950b5fc1e200ull, 0xc5fce83e576d9d24ull, 0x059c805da1c3a4d4ull}); }
 inline U256 omega_of(uint32_t k) { U256 w = root_of_unity(); for (uint32_t i = k; i < 28; i++) w = mulmod(w, w); return w; }
 
 // ---- expressions ----------------------------------------------------------------------------------------------------
@@ -470,9 +479,11 @@ struct DeviceMemory {
   virtual void upload(Fr* dst, const Fr* src, size_t rows) = 0;
   virtual void download(Fr* dst, const Fr* src, size_t rows) = 0;
   virtual void copy(Fr* dst, const Fr* src, size_t rows) = 0;
+  virtual void zero(Fr* p, size_t rows) = 0;
 };
 struct HostMemory : DeviceMemory {                           // "device" = host: the CPU tests' binding (tests/abi_shim)
   Fr* alloc(size_t rows) override { return (Fr*)calloc(rows ? rows : 1, sizeof(Fr)); }
+  void zero(Fr* p, size_t rows) override { memset(p, 0, rows * sizeof(Fr)); }
   void free(Fr* p) override { ::free(p); }
   void upload(Fr* d, const Fr* s, size_t rows) override { memcpy(d, s, rows * sizeof(Fr)); }
   void download(Fr* d, const Fr* s, size_t rows) override { memcpy(d, s, rows * sizeof(Fr)); }
@@ -522,6 +533,7 @@ struct CudaMemory : DeviceMemory {
     ck(cudaMemcpyAsync(d, s, rows * sizeof(Fr), cudaMemcpyDeviceToHost, stream_)); ck(cudaStreamSynchronize(stream_));
   }
   void copy(Fr* d, const Fr* s, size_t rows) override { ck(cudaMemcpyAsync(d, s, rows * sizeof(Fr), cudaMemcpyDeviceToDevice, stream_)); }
+  void zero(Fr* p, size_t rows) override { ck(cudaMemsetAsync(p, 0, rows * sizeof(Fr), stream_)); }
  private:
   cudaStream_t stream_;
   std::map<size_t, std::vector<void*>> free_;
@@ -563,6 +575,7 @@ class Engine {
   Buffer upload(const Fr* host, size_t rows) { Buffer b(mem_, rows); mem_.upload(b.ptr(), host, rows); return b; }
   Buffer clone(const Buffer& b) { Buffer c(mem_, b.rows()); mem_.copy(c.ptr(), b.ptr(), b.rows()); return c; }
   void write_rows(Buffer& b, size_t start, const Fr* rows, size_t count) { if (count) mem_.upload(b.ptr() + start, rows, count); }
+  void zero(Buffer& b) { mem_.zero(b.ptr(), b.rows()); }
 
   std::vector<Point> commit(int basis, const std::vector<const Fr*>& bufs, size_t len) {
     std::vector<spb_g1> jac(bufs.size());
@@ -584,6 +597,18 @@ class Engine {
   Buffer coeff_to_extended(const Buffer& b) { Buffer o(mem_, (size_t)1 << extended_k); check(spb_coeff_to_extended_dev(ctx_, dom_, b.ptr(), o.ptr()), "spb_coeff_to_extended_dev"); return o; }
   Buffer extended_to_coeff(const Buffer& e, size_t rows) { Buffer o(mem_, rows); check(spb_extended_to_coeff_dev(ctx_, dom_, e.ptr(), o.ptr()), "spb_extended_to_coeff_dev"); return o; }
   void divide_by_vanishing(Buffer& e) { check(spb_divide_by_vanishing_dev(ctx_, dom_, e.ptr()), "spb_divide_by_vanishing_dev"); }
+  // the library this program runs against has the three per-part entry points (weak references, see the top of this header)
+  static bool has_per_part() {
+    return spb_coeff_to_extended_part_batch_dev != nullptr && spb_extended_part_scatter_dev != nullptr && spb_permutation_constraints_coset_dev != nullptr;
+  }
+  // outs[i] (n rows) = rows part, part + R, ... of the extended coset of in[i]; the inputs are not written
+  void coeff_to_extended_part_many(const std::vector<const Fr*>& in, uint32_t part, std::vector<Buffer>& outs) {
+    std::vector<Fr*> o; for (auto& b : outs) o.push_back(b.ptr());
+    if (!in.empty()) check(spb_coeff_to_extended_part_batch_dev(ctx_, dom_, part, in.data(), o.data(), in.size()), "spb_coeff_to_extended_part_batch_dev");
+  }
+  void extended_part_scatter(const Buffer& part_values, uint32_t part, Buffer& values) {
+    check(spb_extended_part_scatter_dev(ctx_, dom_, part, part_values.ptr(), values.ptr()), "spb_extended_part_scatter_dev");
+  }
 
   void graph_evaluate(const Graph& g, const std::vector<const Fr*>& fixed, const std::vector<const Fr*>& advice, const std::vector<const Fr*>& instance,
                       const Fr& beta, const Fr& gamma, const Fr& theta, const Fr& y, Buffer& values, uint64_t size, int32_t rot_scale) {
@@ -597,6 +622,14 @@ class Engine {
                                const Fr& beta, const Fr& gamma, const Fr& y, const Fr& ext_omega) {
     check(spb_permutation_constraints_dev(ctx_, values.ptr(), size, rot_scale, last_rotation, (uint32_t)z.size(), chunk_len, z.data(), (uint32_t)cols.size(), cols.data(),
                                           sigma.data(), l0.ptr(), l_last.ptr(), l_active.ptr(), &beta, &gamma, &y, &ext_omega), "spb_permutation_constraints_dev");
+  }
+  // the same terms with X = coset_generator * omega^idx (a coset part of the extended coset)
+  void permutation_constraints_coset(Buffer& values, uint64_t size, int32_t rot_scale, int32_t last_rotation, uint32_t chunk_len, const std::vector<const Fr*>& z,
+                                     const std::vector<const Fr*>& cols, const std::vector<const Fr*>& sigma, const Buffer& l0, const Buffer& l_last,
+                                     const Buffer& l_active, const Fr& beta, const Fr& gamma, const Fr& y, const Fr& coset_generator, const Fr& omega) {
+    check(spb_permutation_constraints_coset_dev(ctx_, values.ptr(), size, rot_scale, last_rotation, (uint32_t)z.size(), chunk_len, z.data(), (uint32_t)cols.size(),
+                                                cols.data(), sigma.data(), l0.ptr(), l_last.ptr(), l_active.ptr(), &beta, &gamma, &y, &coset_generator, &omega),
+          "spb_permutation_constraints_coset_dev");
   }
   void lookup_constraints(Buffer& values, uint64_t size, int32_t rot_scale, const Buffer& product, const Buffer& pin, const Buffer& ptab, const Buffer& table_value,
                           const Buffer& l0, const Buffer& l_last, const Buffer& l_active, const Fr& beta, const Fr& gamma, const Fr& y) {
@@ -657,15 +690,17 @@ using Cell = std::pair<uint32_t, uint64_t>;                  // (index in cs.per
 // cosets stay in device memory with the key. OnDemand (a lean key): the key holds only its n-row data, with the three l
 // polynomials in coefficient form in `l_polys`, and create_proof rebuilds the cosets for each proof and frees them after the
 // quotient. The proof bytes are the same in both modes. CudaMemory keeps the freed cosets on its free lists for the next proof;
-// a process that holds several keys calls trim() after a proof to give them back to the device.
-enum class Cosets { Resident, OnDemand };
+// a process that holds several keys calls trim() after a proof to give them back to the device. PerPart: the key of OnDemand,
+// whose proofs evaluate the quotient one n-row coset part at a time (no column but `values` and the quotient's coefficients
+// has more than n rows; spectre_b200/plonk.py, evaluate_h_per_part).
+enum class Cosets { Resident, OnDemand, PerPart };
 struct ProvingKey {
   ConstraintSystem cs;                                      // held by value (expression nodes are shared_ptr): a cached key never dangles
   uint32_t k = 0; size_t n = 0; uint32_t blinding_factors = 0; size_t usable_rows = 0;
   Cosets cosets = Cosets::Resident;
   std::vector<Buffer> fixed_values, fixed_polys, fixed_cosets, sigma_values, sigma_polys, sigma_cosets;
   Buffer l0, l_last, l_active;                              // Resident only
-  std::vector<Buffer> l_polys;                              // OnDemand only: l0, l_last, l_active in coefficient form
+  std::vector<Buffer> l_polys;                              // OnDemand / PerPart only: l0, l_last, l_active in coefficient form
   std::vector<Point> fixed_commitments, sigma_commitments;
   U256 vk_digest{};
 };
@@ -884,7 +919,54 @@ inline std::vector<uint8_t> create_proof(Engine& E, const ProvingKey& pk, const 
   // 7. quotient
   Buffer h_coeff;
   const uint32_t pieces_n = (uint32_t)cs.degree() - 1;
-  {
+  if (pk.cosets == Cosets::PerPart) {
+    // one coset part at a time (plonk.py evaluate_h_per_part): part j holds the extended rows j + R m, the values at g_j omega^m
+    // with g_j = zeta extended_omega^j, so every pass runs on n rows with rot_scale 1 and only the permutation takes g_j.
+    // Every part buffer is allocated once and released before divide_by_vanishing.
+    if (!Engine::has_per_part())
+      throw std::runtime_error("create_proof: a per-part key needs spb_coeff_to_extended_part_batch_dev, spb_extended_part_scatter_dev and "
+                               "spb_permutation_constraints_coset_dev, which the linked library does not export");
+    const uint32_t R = 1u << (E.extended_k - pk.k);
+    std::vector<const Fr*> srcs = ptrs(pk.fixed_polys);
+    auto add = [&](const std::vector<Buffer>& v) { for (auto& b : v) srcs.push_back(b.ptr()); };
+    add(pk.sigma_polys); add(pk.l_polys); add(advice_polys); add(inst_polys); add(perm_polys);
+    for (auto& l : lookups) { srcs.push_back(l.product.ptr()); srcs.push_back(l.permuted_input_poly.ptr()); srcs.push_back(l.permuted_table_poly.ptr()); }
+    std::vector<Buffer> parts;
+    for (size_t i = 0; i < srcs.size(); i++) parts.push_back(E.alloc(n));
+    size_t at = 0;
+    auto take = [&](size_t count) { std::vector<const Fr*> v; for (size_t i = 0; i < count; i++) v.push_back(parts[at + i].ptr()); at += count; return v; };
+    const std::vector<const Fr*> fixed_p = take(pk.fixed_polys.size()), sigma_p = take(pk.sigma_polys.size());
+    const size_t l_at = at; at += 3;
+    const Buffer &l0 = parts[l_at], &l_last = parts[l_at + 1], &l_active = parts[l_at + 2];
+    const std::vector<const Fr*> advice_p = take(advice_polys.size()), inst_p = take(inst_polys.size()), z_p = take(perm_polys.size());
+    const size_t lookup_at = at;
+    std::vector<const Fr*> cols;
+    for (auto& pc : cs.permutation) cols.push_back((pc.first == Col::Fixed ? fixed_p : pc.first == Col::Advice ? advice_p : inst_p)[pc.second]);
+    U256 ew = root_of_unity(); for (uint32_t i = E.extended_k; i < 28; i++) ew = mulmod(ew, ew);
+    const Fr omega = fr_mont(w);
+    Buffer part_values = E.alloc(n), table_value;
+    if (!lookups.empty()) table_value = E.alloc(n);
+    Buffer values = E.alloc(ext_n);
+    for (uint32_t j = 0; j < R; j++) {
+      E.coeff_to_extended_part_many(srcs, j, parts);
+      if (j) E.zero(part_values);                            // PreviousValue of the gates reads it: every part starts at zero
+      if (!cs.gates.empty()) E.graph_evaluate(cs.gates_program(), fixed_p, advice_p, inst_p, beta, gamma, theta, y, part_values, n, 1);
+      if (!perm_polys.empty()) {
+        const Fr g = fr_mont(mulmod(zeta(), powmod(ew, j)));
+        E.permutation_constraints_coset(part_values, n, 1, -(int32_t)(bf + 1), chunk, z_p, cols, sigma_p, l0, l_last, l_active, beta, gamma, y, g, omega);
+      }
+      for (size_t li = 0; li < lookups.size(); li++) {
+        if (j || li) E.zero(table_value);
+        E.graph_evaluate(cs.lookup_value_program(li), fixed_p, advice_p, inst_p, beta, gamma, theta, zero4, table_value, n, 1);
+        const size_t p0 = lookup_at + 3 * li;
+        E.lookup_constraints(part_values, n, 1, parts[p0], parts[p0 + 1], parts[p0 + 2], table_value, l0, l_last, l_active, beta, gamma, y);
+      }
+      E.extended_part_scatter(part_values, j, values);
+    }
+    parts.clear(); part_values.release(); table_value.release();
+    E.divide_by_vanishing(values);
+    h_coeff = E.extended_to_coeff(values, n * pieces_n);
+  } else {
     // a lean key's cosets are rebuilt here and released with the advice cosets, before divide_by_vanishing
     const bool lean = pk.cosets == Cosets::OnDemand;
     std::vector<Buffer> key_fixed, key_sigma, key_l;

@@ -112,14 +112,6 @@ int stream_device_to_file(spb_ctx* ctx, DeviceState& d, FILE* f, const void* d_s
 
 }  // namespace spb
 
-struct spb_domain {
-  uint32_t j, k, extended_k, quotient_poly_degree;
-  Fr omega, omega_inv, extended_omega, extended_omega_inv, g_coset, g_coset_inv, ifft_divisor, extended_ifft_divisor;
-  uint32_t t_len;
-  Fr* d_t_evaluations;  // device, t_len values
-  int device;
-};
-
 template <class P>
 __global__ void field_op_kernel(int op, const Fp<P>* a, const Fp<P>* b, Fp<P>* o, size_t n) {
   size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
@@ -203,7 +195,7 @@ void spb_shutdown(spb_ctx* ctx) {
     cudaSetDevice(d.device);
     cudaStreamSynchronize(d.stream);
     for (auto& kv : d.slots) if (kv.second.ptr) cudaFree(kv.second.ptr);
-    for (auto& t : d.ntt_tables) { cudaFree(t.tw_lo); cudaFree(t.tw_hi); if (t.tw_full) cudaFree(t.tw_full); }
+    ntt_free_tables(d);
     if (d.pinned) cudaFreeHost(d.pinned);
     for (int i = 0; i < 2; i++) { if (d.stage[i]) cudaFreeHost(d.stage[i]); if (d.stage_done[i]) cudaEventDestroy(d.stage_done[i]); }
     cudaEventDestroy(d.ev0); cudaEventDestroy(d.ev1); cudaEventDestroy(d.dep_ev);
@@ -222,8 +214,7 @@ int spb_release_workspace(spb_ctx* ctx) {
     SPB_CUDA(ctx, cudaDeviceSynchronize());
     for (auto& kv : d.slots) if (kv.second.ptr) cudaFree(kv.second.ptr);
     d.slots.clear();
-    for (auto& t : d.ntt_tables) { cudaFree(t.tw_lo); cudaFree(t.tw_hi); if (t.tw_full) cudaFree(t.tw_full); }
-    d.ntt_tables.clear();
+    ntt_free_tables(d);
   }
   if (!ctx->dev.empty()) cudaSetDevice(ctx->dev[0].device);
   return 0;
@@ -485,6 +476,16 @@ int spb_coeff_to_extended_batch_dev(spb_ctx* ctx, const spb_domain* dm, const sp
   std::lock_guard<std::mutex> lk(ctx->mu);
   Fr pre[3]; NttOpts o; c2e_opts(dm, pre, o);
   return ntt_batch_devices(ctx, d_in, d_out, count, dm->extended_k, dm->extended_omega, o);
+}
+// Coset part `part` of the extended coset: the extended rows part + R m (R = 2^(extended_k - k)) are the values at
+// g omega^m with g = zeta extended_omega^part, so they are the n-point transform of the coefficients pre-scaled by g^a.
+int spb_coeff_to_extended_part_batch_dev(spb_ctx* ctx, const spb_domain* dm, uint32_t part, const spb_fr* const* d_in, spb_fr* const* d_out, size_t count) {
+  if (!ctx || !dm || (count && (!d_in || !d_out))) return SPB_ERR_ARG;
+  if (part >= dm->t_len) return set_error(ctx, SPB_ERR_ARG, "spb_coeff_to_extended_part_batch_dev: part %u of %u", part, dm->t_len);
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  const Fr g = fp_mul(dm->g_coset, fp_pow_u64(dm->extended_omega, part));
+  NttOpts o; o.pre_generator = &g;
+  return ntt_batch_devices(ctx, d_in, d_out, count, dm->k, dm->omega, o);
 }
 int spb_divide_by_vanishing_dev(spb_ctx* ctx, const spb_domain* dm, spb_fr* d_a) {
   if (!ctx || !dm || !d_a) return SPB_ERR_ARG;

@@ -52,6 +52,7 @@ struct DeviceState {
   std::map<std::string, DevBuf> slots;
   MsmLane lanes[kMaxMsmLanes];   // created on first use, released with the context (all access under the context lock)
   std::vector<NttTables> ntt_tables;
+  std::vector<NttTables> ntt_pre_tables;  // power tables of coset generators (NttOpts::pre_generator; never a full table)
   void* pinned = nullptr;  // small pinned staging area for results
   size_t pinned_cap = 0;
   void* stage[2] = {nullptr, nullptr};              // two pinned 16 MiB buffers for file <-> device streaming (lazily allocated)
@@ -71,6 +72,15 @@ struct spb_ctx {
   uint64_t last_msm_adds = 0;  // G1 additions of the last MSM call / batch
   bool shplonk_slots_busy = false;  // the context's SHPLONK workspace slots are held by an open spb_shplonk handle
   float msm_stage_ms[7] = {0, 0, 0, 0, 0, 0, 0};  // count, scan, scatter, accumulate, stitch, segment, window (device 0)
+};
+
+// EvaluationDomain (capi.cu builds it; quotient.cu reads its sizes)
+struct spb_domain {
+  uint32_t j, k, extended_k, quotient_poly_degree;
+  spb::Fr omega, omega_inv, extended_omega, extended_omega_inv, g_coset, g_coset_inv, ifft_divisor, extended_ifft_divisor;
+  uint32_t t_len;
+  spb::Fr* d_t_evaluations;  // device, t_len values
+  int device;
 };
 
 namespace spb {
@@ -164,7 +174,10 @@ struct NttOpts {
   uint64_t n_in = 0, n_out = 0;  // 0 = n
   const Fr* pre3 = nullptr;      // host pointers to 3 factors, or nullptr
   const Fr* post3 = nullptr;
+  const Fr* pre_generator = nullptr;  // host pointer to g, or nullptr: input i multiplied by g^i (power tables cached per (k, g))
 };
+// free every table of a device's NTT caches (the caller has synchronised the device)
+void ntt_free_tables(DeviceState& d);
 // d_src/d_dst device pointers (may alias); omega host value (Montgomery)
 int ntt_device(spb_ctx* ctx, DeviceState& d, const Fr* d_src, Fr* d_dst, uint32_t log_n, const Fr& omega, const NttOpts& opts);
 // several devices in the context: six-step across devices with one all-to-all (host buffers)

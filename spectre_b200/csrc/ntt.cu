@@ -19,8 +19,11 @@ static const size_t kFullTableBudget = (size_t)6 << 30;
 
 static NttPlan make_plan(uint32_t k) { return ntt_make_plan(k, kMaxDigitBits); }
 
-static int get_tables(spb_ctx* ctx, DeviceState& d, uint32_t k, const Fr& omega, uint32_t h, NttTables** out) {
-  for (auto& t : d.ntt_tables)
+// Power tables of `omega` split at h, cached per (k, omega, h) in `cache`: the twiddle tables (d.ntt_tables, with a full table
+// while the budget allows) or the pre-scale tables of coset generators (d.ntt_pre_tables, two-level only). The two caches are
+// separate, so fetching one kind never evicts a table of the other kind that the same transform is about to use.
+static int get_tables(spb_ctx* ctx, DeviceState& d, std::vector<NttTables>& cache, uint32_t k, const Fr& omega, uint32_t h, bool full_allowed, NttTables** out) {
+  for (auto& t : cache)
     if (t.k == k && t.h == h && fp_eq(t.omega, omega)) { *out = &t; return 0; }
   NttTables t; t.omega = omega; t.k = k; t.h = h;
   size_t nlo = (size_t)1 << h, nhi = (size_t)1 << (k - h);
@@ -28,9 +31,9 @@ static int get_tables(spb_ctx* ctx, DeviceState& d, uint32_t k, const Fr& omega,
   SPB_CUDA(ctx, cudaMalloc(&t.tw_hi, nhi * sizeof(Fr)));
   SPB_TRY(launch(ctx, d.stream, nblk(nlo, 128), 128, 0, fr_pow_table_kernel, t.tw_lo, omega, nlo, 0));
   SPB_TRY(launch(ctx, d.stream, nblk(nhi, 128), 128, 0, fr_pow_table_kernel, t.tw_hi, omega, nhi, h));
-  {
+  if (full_allowed) {
     size_t used = 0;
-    for (auto& o : d.ntt_tables) if (o.tw_full) used += ((size_t)1 << o.k) * sizeof(Fr);
+    for (auto& o : cache) if (o.tw_full) used += ((size_t)1 << o.k) * sizeof(Fr);
     size_t need = ((size_t)1 << k) * sizeof(Fr);
     if (k >= 12 && used + need <= kFullTableBudget && cudaMalloc(&t.tw_full, need) == cudaSuccess) {
       SPB_TRY(launch(ctx, d.stream, nblk((uint64_t)1 << k, 128), 128, 0, fr_pow_table_kernel, t.tw_full, omega, (uint64_t)1 << k, 0));
@@ -40,22 +43,30 @@ static int get_tables(spb_ctx* ctx, DeviceState& d, uint32_t k, const Fr& omega,
     }
   }
   // a long-lived prover touches a handful of (k, omega) pairs; cap the cache anyway
-  if (d.ntt_tables.size() >= 32) {
+  if (cache.size() >= 32) {
     cudaStreamSynchronize(d.stream);
-    cudaFree(d.ntt_tables.front().tw_lo); cudaFree(d.ntt_tables.front().tw_hi); if (d.ntt_tables.front().tw_full) cudaFree(d.ntt_tables.front().tw_full);
-    d.ntt_tables.erase(d.ntt_tables.begin());
+    cudaFree(cache.front().tw_lo); cudaFree(cache.front().tw_hi); if (cache.front().tw_full) cudaFree(cache.front().tw_full);
+    cache.erase(cache.begin());
   }
-  d.ntt_tables.push_back(t);
-  *out = &d.ntt_tables.back();
+  cache.push_back(t);
+  *out = &cache.back();
   return 0;
+}
+
+void ntt_free_tables(DeviceState& d) {
+  for (auto* cache : {&d.ntt_tables, &d.ntt_pre_tables}) {
+    for (auto& t : *cache) { cudaFree(t.tw_lo); cudaFree(t.tw_hi); if (t.tw_full) cudaFree(t.tw_full); }
+    cache->clear();
+  }
 }
 
 // Geometry of pass `pi` (ntt_fill_pass, shared with the host emulation) and its launch.
 static int launch_pass(spb_ctx* ctx, DeviceState& d, const NttPlan& plan, uint32_t pi, uint32_t k, const NttTables* tb, uint32_t h,
-                       const Fr* src, Fr* dst, const NttOpts& opts, const NttShare& sh) {
+                       const Fr* src, Fr* dst, const NttOpts& opts, const NttShare& sh, const NttTables* pre = nullptr) {
   NttPassParams p;
   p.src = src; p.dst = dst; p.tw_lo = tb->tw_lo; p.tw_hi = tb->tw_hi; p.tw_full = tb->tw_full;
   NttOptsHost oh; oh.n_in = opts.n_in; oh.n_out = opts.n_out; oh.pre3 = opts.pre3; oh.post3 = opts.post3;
+  if (pre) { oh.pre_lo = pre->tw_lo; oh.pre_hi = pre->tw_hi; }
   NttLaunch L = ntt_fill_pass(p, plan, pi, k, h, oh, sh, tile_elems_log(k), kPassThreads);
   if (L.smem > 227 * 1024) return set_error(ctx, SPB_ERR_STATE, "ntt: tile needs %zu B of shared memory", L.smem);
   // persistent CTAs: as many as fit the SMs (shared memory bound), striding over the tiles
@@ -85,7 +96,9 @@ int ntt_device(spb_ctx* ctx, DeviceState& d, const Fr* d_src, Fr* d_dst, uint32_
   NttPlan plan = make_plan(k);
   uint32_t h = k - plan.s[0];
   NttTables* tb = nullptr;
-  SPB_TRY(get_tables(ctx, d, k, omega, h, &tb));
+  NttTables* pre = nullptr;
+  SPB_TRY(get_tables(ctx, d, d.ntt_tables, k, omega, h, true, &tb));
+  if (opts.pre_generator) SPB_TRY(get_tables(ctx, d, d.ntt_pre_tables, k, *opts.pre_generator, h, false, &pre));
   Fr* tmp = nullptr;
   if (plan.npass > 1) {
     tmp = (Fr*)slot(ctx, d, "ntt_tmp", n * sizeof(Fr));
@@ -95,7 +108,7 @@ int ntt_device(spb_ctx* ctx, DeviceState& d, const Fr* d_src, Fr* d_dst, uint32_
   for (uint32_t pi = 0; pi < plan.npass; pi++) {
     const Fr* src = (pi == 0) ? d_src : tmp;
     Fr* dst = (pi == plan.npass - 1) ? d_dst : tmp;
-    SPB_TRY(launch_pass(ctx, d, plan, pi, k, tb, h, src, dst, opts, NttShare()));
+    SPB_TRY(launch_pass(ctx, d, plan, pi, k, tb, h, src, dst, opts, NttShare(), pre));
   }
   return 0;
 }
@@ -135,7 +148,7 @@ int ntt_multi_host(spb_ctx* ctx, const Fr* in, Fr* out, uint32_t k, const Fr& om
     A[q] = (Fr*)slot(ctx, d, "ntt_md_a", per * sizeof(Fr));
     B[q] = (Fr*)slot(ctx, d, "ntt_md_b", per * sizeof(Fr));
     if (!A[q] || !B[q]) return SPB_ERR_OOM;
-    SPB_TRY(get_tables(ctx, d, k, omega, h, &tbs[q]));
+    SPB_TRY(get_tables(ctx, d, d.ntt_tables, k, omega, h, true, &tbs[q]));
     SPB_TRY(set_smem_attr(ctx, d));
     // 1. column block q of the first rows_in rows
     if (rows_in) SPB_CUDA(ctx, cudaMemcpy2DAsync(A[q], lo_loc * sizeof(Fr), in + q * lo_loc, lo_count * sizeof(Fr), lo_loc * sizeof(Fr), rows_in, cudaMemcpyHostToDevice, d.stream));

@@ -52,9 +52,11 @@ struct NttPassParams {
   uint32_t out_local;   // last pass: store at (o >> s1) * 2^out_cols_log + (i_1 - i1_base) instead of o
   uint32_t out_cols_log;
   uint32_t i1_base;
-  uint32_t use_pre, use_post;
+  uint32_t use_pre, use_post;   // use_pre: 1 = pre[i % 3], 2 = the power table g^i below
   uint64_t n_in;     // elements >= n_in of the input are zero (not read)
   uint64_t n_out;    // only outputs < n_out are stored
+  const Fr* pre_lo;  // g^i,          i < 2^h    (use_pre == 2: input i multiplied by g^i in the first pass)
+  const Fr* pre_hi;  // g^(i * 2^h),  i < 2^(k-h)
   Fr pre[3];         // input i multiplied by pre[i % 3]   (first pass)
   Fr post[3];        // output i multiplied by post[i % 3] (last pass)
 };
@@ -154,6 +156,14 @@ SPB_HD Fr ntt_omega_pow(const NttPassParams& p, uint64_t e) {
   if (hi == 0) return wl;
   return fp_mul(ntt_ldg(p.tw_hi + hi), wl);
 }
+// g^e through the two-level power table of the pre-scale (the same split h as the twiddles)
+SPB_HD Fr ntt_pre_pow(const NttPassParams& p, uint64_t e) {
+  uint64_t hi = e >> p.h, lo = e & ((1ull << p.h) - 1);
+  if (lo == 0) return ntt_ldg(p.pre_hi + hi);
+  Fr wl = ntt_ldg(p.pre_lo + lo);
+  if (hi == 0) return wl;
+  return fp_mul(ntt_ldg(p.pre_hi + hi), wl);
+}
 
 // ---- one tile, written as barrier-separated phases over (tid, T) so that tests/hostemu can run the identical code
 // ---- serially (every phase for all tid, then the next phase) and the kernel runs it with __syncthreads between.
@@ -182,7 +192,7 @@ SPB_HD void ntt_phase_twiddles(const NttPassParams& p, const NttSmem& sm, uint32
   const uint32_t S = 1u << p.s;
   for (uint32_t j = tid; j < (S >> 1); j += T) sm.set_twiddle(j, ntt_omega_pow(p, (uint64_t)j << (p.k - p.s)));
 }
-// load the tile (natural order), fusing zero padding and the zeta-coset pre-scale
+// load the tile (natural order), fusing zero padding and the pre-scale (zeta-coset factors, or powers of a coset generator)
 SPB_HD void ntt_phase_load(const NttPassParams& p, const NttSmem& sm, const NttTile& t, uint32_t tid, uint32_t T) {
   const uint32_t S = 1u << p.s, C = 1u << p.logc;
   for (uint32_t e = tid; e < S * C; e += T) {
@@ -198,7 +208,8 @@ SPB_HD void ntt_phase_load(const NttPassParams& p, const NttSmem& sm, const NttT
     if (p.first && gglob >= p.n_in) v = fp_zero<FrParams>();
     else {
       v = ntt_ld_stream(p.src + gi);
-      if (p.first && p.use_pre) { uint32_t m = (uint32_t)(gglob % 3); if (m) v = fp_mul(v, p.pre[m]); }
+      if (p.first && p.use_pre == 1) { uint32_t m = (uint32_t)(gglob % 3); if (m) v = fp_mul(v, p.pre[m]); }
+      else if (p.first && p.use_pre == 2 && gglob) v = fp_mul(v, ntt_pre_pow(p, gglob));
     }
     sm.store(c, r, v);
   }
@@ -282,6 +293,8 @@ struct NttOptsHost {   // what EvaluationDomain fuses around the transform
   uint64_t n_in = 0, n_out = 0;  // 0 = n
   const Fr* pre3 = nullptr;      // 3 factors, or nullptr
   const Fr* post3 = nullptr;
+  const Fr* pre_lo = nullptr;    // two-level power table of g (split h of the plan), or nullptr: input i multiplied by g^i
+  const Fr* pre_hi = nullptr;
 };
 struct NttLaunch { uint64_t tiles; uint32_t threads; size_t smem; };
 // Fill everything of pass `pi` except the pointers (src, dst, twiddle tables).
@@ -299,6 +312,7 @@ inline NttLaunch ntt_fill_pass(NttPassParams& p, const NttPlan& plan, uint32_t p
   p.n_in = opts.n_in ? opts.n_in : n;
   p.n_out = opts.n_out ? opts.n_out : n;
   if (p.first && opts.pre3) { p.use_pre = 1; for (int i = 0; i < 3; i++) p.pre[i] = opts.pre3[i]; }
+  if (p.first && opts.pre_lo) { p.use_pre = 2; p.pre_lo = opts.pre_lo; p.pre_hi = opts.pre_hi; }
   if (p.last && opts.post3) { p.use_post = 1; for (int i = 0; i < 3; i++) p.post[i] = opts.post3[i]; }
   p.b_addr = p.b;
   // columns per tile: as many as fit, bounded by what the direction offers on this device

@@ -41,6 +41,11 @@ __global__ void __launch_bounds__(256) lookup_constraints_kernel(LookupArgs a) {
   if (idx < a.row_hi) lookup_constraints_row(a, idx);
 }
 
+__global__ void __launch_bounds__(256) extended_part_scatter_kernel(const Fr* part_values, Fr* extended, uint32_t part, uint32_t R, uint64_t row_lo, uint64_t row_hi) {
+  uint64_t m = row_lo + blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+  if (m < row_hi) extended_part_scatter_row(part_values, extended, part, R, m);
+}
+
 namespace {
 
 // Each pass runs in row-range shards over `size` extended rows (row_ranges; SURVEY.md 8e "evaluate_h / pointwise":
@@ -178,6 +183,44 @@ bool schedule_program(const uint32_t* words, size_t nwords, uint32_t ncalc, std:
   return true;
 }
 
+// The permutation pass with X = g * omega^idx at row idx: (zeta, extended_omega) over the whole extended coset, (zeta
+// extended_omega^j, omega) over its coset part j.
+int permutation_constraints(spb_ctx* ctx, spb_fr* d_values, uint64_t size, int32_t rot_scale, int32_t last_rotation, uint32_t n_sets, uint32_t chunk_len,
+                            const spb_fr* const* d_z, uint32_t n_cols, const spb_fr* const* d_col_values, const spb_fr* const* d_sigma,
+                            const spb_fr* d_l0, const spb_fr* d_l_last, const spb_fr* d_l_active, const spb_fr* beta, const spb_fr* gamma,
+                            const spb_fr* y, const Fr& g, const Fr& omega) {
+  if (!size || (size & (size - 1))) return set_error(ctx, SPB_ERR_ARG, "permutation constraints: the domain size must be a power of two");
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  DeviceState& d = ctx->dev[0];
+  SPB_CUDA(ctx, cudaSetDevice(d.device));
+  SPB_CUDA(ctx, cudaEventRecord(d.ev0, d.stream));
+  if (ctx->dev.size() > 1) SPB_CUDA(ctx, cudaEventRecord(d.dep_ev, d.stream));
+  PermArgs a; memset(&a, 0, sizeof a);
+  a.values = (Fr*)d_values; a.size = size; a.rot_scale = rot_scale; a.last_rotation = last_rotation;
+  a.n_sets = n_sets; a.chunk_len = chunk_len; a.n_cols = n_cols;
+  a.l0 = (const Fr*)d_l0; a.l_last = (const Fr*)d_l_last; a.l_active = (const Fr*)d_l_active;
+  a.beta = fr_load(beta); a.gamma = fr_load(gamma); a.y = fr_load(y); a.extended_omega = omega;
+  a.delta = fr_delta();
+  a.delta_start = fp_mul(a.beta, g);
+  std::vector<Fr> pw(256);
+  pw[0] = fp_one<FrParams>();
+  for (int j = 1; j < 256; j++) pw[j] = fp_mul(pw[j - 1], a.extended_omega);
+  const std::vector<RowRange> shards = row_ranges(ctx, size);
+  for (auto& sh : shards) {
+    DeviceState& dv = ctx->dev[sh.dev_index];
+    SPB_TRY(shard_begin(ctx, sh));
+    a.z = upload_ptrs(ctx, dv, "q_z", d_z, n_sets);
+    a.col_values = upload_ptrs(ctx, dv, "q_cols", d_col_values, n_cols);
+    a.sigma = upload_ptrs(ctx, dv, "q_sigma", d_sigma, n_cols);
+    Fr* dpw = (Fr*)slot(ctx, dv, "q_omega_pow", 256 * sizeof(Fr));
+    if (!a.z || !a.col_values || !a.sigma || !dpw) return set_error(ctx, SPB_ERR_CUDA, "permutation: table upload failed");
+    SPB_CUDA(ctx, cudaMemcpyAsync(dpw, pw.data(), 256 * sizeof(Fr), cudaMemcpyHostToDevice, dv.stream));
+    a.omega_pow = dpw; a.row_lo = sh.lo; a.row_hi = sh.hi;
+    SPB_TRY(launch(ctx, dv.stream, nblk(sh.hi - sh.lo, 256), 256, 0, permutation_constraints_kernel, a));
+  }
+  return shards_finish(ctx, shards);
+}
+
 }  // namespace
 
 extern "C" {
@@ -255,30 +298,30 @@ int spb_permutation_constraints_dev(spb_ctx* ctx, spb_fr* d_values, uint64_t siz
   if (!ctx || !d_values || !beta || !gamma || !y || !extended_omega || !d_l0 || !d_l_last || !d_l_active) return SPB_ERR_ARG;
   if (!n_sets) return 0;
   if (!d_z || !chunk_len || (n_cols && (!d_col_values || !d_sigma))) return SPB_ERR_ARG;
-  if (!size || (size & (size - 1))) return set_error(ctx, SPB_ERR_ARG, "permutation constraints: the extended domain size must be a power of two");
+  return permutation_constraints(ctx, d_values, size, rot_scale, last_rotation, n_sets, chunk_len, d_z, n_cols, d_col_values, d_sigma, d_l0, d_l_last,
+                                 d_l_active, beta, gamma, y, fr_zeta(), fr_load(extended_omega));
+}
+
+int spb_permutation_constraints_coset_dev(spb_ctx* ctx, spb_fr* d_values, uint64_t size, int32_t rot_scale, int32_t last_rotation, uint32_t n_sets,
+                                          uint32_t chunk_len, const spb_fr* const* d_z, uint32_t n_cols, const spb_fr* const* d_col_values,
+                                          const spb_fr* const* d_sigma, const spb_fr* d_l0, const spb_fr* d_l_last, const spb_fr* d_l_active,
+                                          const spb_fr* beta, const spb_fr* gamma, const spb_fr* y, const spb_fr* coset_generator, const spb_fr* omega) {
+  if (!ctx || !d_values || !beta || !gamma || !y || !coset_generator || !omega || !d_l0 || !d_l_last || !d_l_active) return SPB_ERR_ARG;
+  if (!n_sets) return 0;
+  if (!d_z || !chunk_len || (n_cols && (!d_col_values || !d_sigma))) return SPB_ERR_ARG;
+  return permutation_constraints(ctx, d_values, size, rot_scale, last_rotation, n_sets, chunk_len, d_z, n_cols, d_col_values, d_sigma, d_l0, d_l_last,
+                                 d_l_active, beta, gamma, y, fr_load(coset_generator), fr_load(omega));
+}
+
+int spb_extended_part_scatter_dev(spb_ctx* ctx, const spb_domain* dm, uint32_t part, const spb_fr* d_part, spb_fr* d_extended) {
+  if (!ctx || !dm || !d_part || !d_extended) return SPB_ERR_ARG;
+  if (part >= dm->t_len) return set_error(ctx, SPB_ERR_ARG, "spb_extended_part_scatter_dev: part %u of %u", part, dm->t_len);
   SPB_ENTER0(ctx);
-  PermArgs a; memset(&a, 0, sizeof a);
-  a.values = (Fr*)d_values; a.size = size; a.rot_scale = rot_scale; a.last_rotation = last_rotation;
-  a.n_sets = n_sets; a.chunk_len = chunk_len; a.n_cols = n_cols;
-  a.l0 = (const Fr*)d_l0; a.l_last = (const Fr*)d_l_last; a.l_active = (const Fr*)d_l_active;
-  a.beta = fr_load(beta); a.gamma = fr_load(gamma); a.y = fr_load(y); a.extended_omega = fr_load(extended_omega);
-  a.delta = fr_delta();
-  a.delta_start = fp_mul(a.beta, fr_zeta());
-  std::vector<Fr> pw(256);
-  pw[0] = fp_one<FrParams>();
-  for (int j = 1; j < 256; j++) pw[j] = fp_mul(pw[j - 1], a.extended_omega);
-  const std::vector<RowRange> shards = row_ranges(ctx, size);
+  const std::vector<RowRange> shards = row_ranges(ctx, 1ull << dm->k);
   for (auto& sh : shards) {
-    DeviceState& dv = ctx->dev[sh.dev_index];
     SPB_TRY(shard_begin(ctx, sh));
-    a.z = upload_ptrs(ctx, dv, "q_z", d_z, n_sets);
-    a.col_values = upload_ptrs(ctx, dv, "q_cols", d_col_values, n_cols);
-    a.sigma = upload_ptrs(ctx, dv, "q_sigma", d_sigma, n_cols);
-    Fr* dpw = (Fr*)slot(ctx, dv, "q_omega_pow", 256 * sizeof(Fr));
-    if (!a.z || !a.col_values || !a.sigma || !dpw) return set_error(ctx, SPB_ERR_CUDA, "permutation: table upload failed");
-    SPB_CUDA(ctx, cudaMemcpyAsync(dpw, pw.data(), 256 * sizeof(Fr), cudaMemcpyHostToDevice, dv.stream));
-    a.omega_pow = dpw; a.row_lo = sh.lo; a.row_hi = sh.hi;
-    SPB_TRY(launch(ctx, dv.stream, nblk(sh.hi - sh.lo, 256), 256, 0, permutation_constraints_kernel, a));
+    SPB_TRY(launch(ctx, ctx->dev[sh.dev_index].stream, nblk(sh.hi - sh.lo, 256), 256, 0, extended_part_scatter_kernel, (const Fr*)d_part, (Fr*)d_extended,
+                   part, dm->t_len, sh.lo, sh.hi));
   }
   return shards_finish(ctx, shards);
 }

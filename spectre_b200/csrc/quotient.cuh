@@ -76,6 +76,8 @@ struct PermArgs {
   const Fr* omega_pow;       // extended_omega^j, j < 256 (device table): omega^idx = omega^(idx & ~255) * omega_pow[idx & 255]
   const Fr* const* z; const Fr* const* col_values; const Fr* const* sigma;
   const Fr* l0; const Fr* l_last; const Fr* l_active;
+  // X at row idx is g * extended_omega^idx: delta_start = beta * g (g = zeta on the whole extended coset, zeta extended_omega^j
+  // with extended_omega = omega on its coset part j)
   Fr beta, gamma, y, delta_start, delta, extended_omega;
 };
 
@@ -126,6 +128,11 @@ SPB_HD void lookup_constraints_row(const LookupArgs& a, uint64_t idx) {
   v = fp_add(fp_mul(v, a.y), fp_mul(a_minus_s, l0));
   v = fp_add(fp_mul(v, a.y), fp_mul(fp_mul(a_minus_s, fp_sub(a_in, ntt_ldg(a.permuted_input + r_prev))), l_active));
   ntt_stg(a.values + idx, v);
+}
+
+// one row of a coset part back into the extended buffer: row m of part `part` is extended row part + R m
+SPB_HD void extended_part_scatter_row(const Fr* part_values, Fr* extended, uint32_t part, uint32_t R, uint64_t m) {
+  ntt_stg(extended + part + (uint64_t)R * m, ntt_ld_stream(part_values + m));
 }
 
 // ---- argument-prover terms (plonk.cu) --------------------------------------------------------------------------------

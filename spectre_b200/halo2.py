@@ -283,6 +283,15 @@ class Backend:
                                                             _p(d_l_active), _p(_fr_array(beta, 1)), _p(_fr_array(gamma, 1)), _p(_fr_array(y, 1)),
                                                             _p(_fr_array(extended_omega, 1))), "spb_permutation_constraints_dev")
 
+    def permutation_constraints_coset_dev(self, d_values, size, rot_scale, last_rotation, chunk_len, d_z, d_col_values, d_sigma, d_l0, d_l_last, d_l_active,
+                                          beta, gamma, y, coset_generator, omega):
+        """permutation_constraints_dev with X = coset_generator * omega^idx at row idx (a coset part of the extended coset)"""
+        mk = lambda ps: (ctypes.c_void_p * max(1, len(ps)))(*ps)
+        self.check(self.lib.spb_permutation_constraints_coset_dev(self.ctx, _p(d_values), ctypes.c_uint64(size), ctypes.c_int32(rot_scale), ctypes.c_int32(last_rotation),
+                                                                  len(d_z), chunk_len, mk(d_z), len(d_col_values), mk(d_col_values), mk(d_sigma), _p(d_l0), _p(d_l_last),
+                                                                  _p(d_l_active), _p(_fr_array(beta, 1)), _p(_fr_array(gamma, 1)), _p(_fr_array(y, 1)),
+                                                                  _p(_fr_array(coset_generator, 1)), _p(_fr_array(omega, 1))), "spb_permutation_constraints_coset_dev")
+
     def lookup_constraints_dev(self, d_values, size, rot_scale, d_product, d_permuted_input, d_permuted_table, d_table_value, d_l0, d_l_last, d_l_active,
                                beta, gamma, y):
         self.check(self.lib.spb_lookup_constraints_dev(self.ctx, _p(d_values), ctypes.c_uint64(size), ctypes.c_int32(rot_scale), _p(d_product), _p(d_permuted_input),
@@ -431,6 +440,17 @@ class EvaluationDomain:
     def coeff_to_extended_batch_dev(self, d_in, d_out):
         pi = (ctypes.c_void_p * max(1, len(d_in)))(*d_in); po = (ctypes.c_void_p * max(1, len(d_out)))(*d_out)
         self.be.check(self.be.lib.spb_coeff_to_extended_batch_dev(self.be.ctx, self.h, pi, po, ctypes.c_size_t(len(d_in))), "spb_coeff_to_extended_batch_dev")
+
+    def coeff_to_extended_part_batch_dev(self, part, d_in, d_out):
+        """d_out[i] = rows part, part + R, part + 2R, ... of coeff_to_extended(d_in[i]) (2^k of them), R = 2^(extended_k - k)"""
+        pi = (ctypes.c_void_p * max(1, len(d_in)))(*d_in); po = (ctypes.c_void_p * max(1, len(d_out)))(*d_out)
+        self.be.check(self.be.lib.spb_coeff_to_extended_part_batch_dev(self.be.ctx, self.h, ctypes.c_uint32(part), pi, po, ctypes.c_size_t(len(d_in))),
+                      "spb_coeff_to_extended_part_batch_dev")
+
+    def extended_part_scatter_dev(self, part, d_part, d_extended):
+        """d_extended[part + R m] = d_part[m] for m < 2^k"""
+        self.be.check(self.be.lib.spb_extended_part_scatter_dev(self.be.ctx, self.h, ctypes.c_uint32(part), _p(d_part), _p(d_extended)),
+                      "spb_extended_part_scatter_dev")
 
     def coeff_to_extended_dev(self, d_in, d_out):
         self.be.check(self.be.lib.spb_coeff_to_extended_dev(self.be.ctx, self.h, _p(d_in), _p(d_out)), "spb_coeff_to_extended_dev")

@@ -27,6 +27,7 @@ _MONT = (1 << 256) % R_MOD
 _MONT_INV = pow(_MONT, -1, R_MOD)
 ROOT_OF_UNITY = pow(7, (R_MOD - 1) >> 28, R_MOD)
 DELTA = pow(7, 1 << 28, R_MOD)
+ZETA = pow(pow(7, (R_MOD - 1) // 3, R_MOD), 2, R_MOD)       # the extended coset's shift (EvaluationDomain g_coset)
 
 # flat GraphEvaluator encoding (include/spectre_b200.h)
 ADD, SUB, MUL, SQUARE, DOUBLE, NEGATE, HORNER, STORE = range(8)
@@ -302,6 +303,14 @@ class DeviceEngine:
         if bufs:
             self.dom.coeff_to_extended_batch_dev([b.data_ptr() for b in bufs], [o.data_ptr() for o in outs])
         return outs
+    def coeff_to_extended_part_many(self, bufs, part, outs):
+        """outs[i] (n rows each) = rows part, part + R, ... of bufs[i]'s extended coset; the inputs are not written"""
+        if bufs:
+            self.dom.coeff_to_extended_part_batch_dev(part, [b.data_ptr() for b in bufs], [o.data_ptr() for o in outs])
+    def extended_part_scatter(self, part_buf, part, values): self.dom.extended_part_scatter_dev(part, part_buf.data_ptr(), values.data_ptr())
+    def zero(self, b):
+        with self.torch.cuda.stream(self.stream):
+            b.zero_()
     def coeff_to_lagrange(self, b):
         self.be.best_fft_dev(b.data_ptr(), fr_mont(omega_of(self.k)).reshape(1, 4), self.k)
     def coeff_to_extended(self, b):
@@ -319,10 +328,16 @@ class DeviceEngine:
         ptr = lambda bs: [b.data_ptr() for b in bs]
         self.be.graph_evaluate_dev(p["prog"], p["ncalc"], p["ncalc"], p["constants"], p["rotations"], ptr(fixed), ptr(advice), ptr(instance),
                                    np.zeros((1, 4), np.uint64), beta, gamma, theta, y, values.data_ptr(), size, rot_scale)
-    def permutation_constraints(self, values, size, rot_scale, last_rotation, chunk_len, z, cols, sigma, l0, l_last, l_active, beta, gamma, y, ext_omega):
+    def permutation_constraints(self, values, size, rot_scale, last_rotation, chunk_len, z, cols, sigma, l0, l_last, l_active, beta, gamma, y, ext_omega,
+                                coset_generator=None):
+        """X = zeta * ext_omega^idx at row idx, or coset_generator * ext_omega^idx when a generator is given (a coset part)"""
         ptr = lambda bs: [b.data_ptr() for b in bs]
-        self.be.permutation_constraints_dev(values.data_ptr(), size, rot_scale, last_rotation, chunk_len, ptr(z), ptr(cols), ptr(sigma), l0.data_ptr(),
-                                            l_last.data_ptr(), l_active.data_ptr(), beta, gamma, y, ext_omega)
+        args = (values.data_ptr(), size, rot_scale, last_rotation, chunk_len, ptr(z), ptr(cols), ptr(sigma), l0.data_ptr(), l_last.data_ptr(), l_active.data_ptr(),
+                beta, gamma, y)
+        if coset_generator is None:
+            self.be.permutation_constraints_dev(*args, ext_omega)
+        else:
+            self.be.permutation_constraints_coset_dev(*args, coset_generator, ext_omega)
     def lookup_constraints(self, values, size, rot_scale, product, pin, ptab, table_value, l0, l_last, l_active, beta, gamma, y):
         self.be.lookup_constraints_dev(values.data_ptr(), size, rot_scale, product.data_ptr(), pin.data_ptr(), ptab.data_ptr(), table_value.data_ptr(),
                                        l0.data_ptr(), l_last.data_ptr(), l_active.data_ptr(), beta, gamma, y)
@@ -379,12 +394,18 @@ def coeff_to_extended_many(E, bufs):
 # only the n-row data -- fixed / sigma values and polys, and the three l polynomials in coefficient form -- and create_proof
 # rebuilds the cosets before the quotient and frees them after it. A rebuilt coset is the same coset, so the proof bytes are
 # the same in both modes; a lean key costs one coset NTT per fixed / sigma / l column per proof.
-COSETS_MODES = ("resident", "on_demand")
+# "per_part" holds what an on_demand key holds, and its proofs evaluate the quotient one coset part at a time: the extended
+# rows part + R m (m < n, R = 2^(extended_k - k)) of every column are built as n-row buffers, evaluated and scattered into the
+# one extended `values`, so no column but `values` and the quotient's coefficients ever has more than n rows. It trades more,
+# smaller transforms for a peak that is about one extended buffer instead of one per column; the proof bytes are the same.
+COSETS_MODES = ("resident", "on_demand", "per_part")
 
 
 class ProvingKey:
-    """A lean key (cosets="on_demand") has fixed_cosets = sigma_cosets = l0 = l_last = l_active = None and holds `l_polys`
-    = [l0, l_last, l_active] in coefficient form instead (None in a resident key)."""
+    """A lean key (cosets="on_demand" or "per_part") has fixed_cosets = sigma_cosets = l0 = l_last = l_active = None and holds
+    `l_polys` = [l0, l_last, l_active] in coefficient form instead (None in a resident key)."""
+
+    per_part = False                                         # cosets="per_part": create_proof evaluates the quotient per coset part
 
     @property
     def lean(self):
@@ -393,7 +414,7 @@ class ProvingKey:
 
 def key_device_bytes(cs, k, extended_k, cosets="resident"):
     """Device bytes a proving key of this shape holds (DESIGN.md section 3), with C = num_fixed + len(permutation) columns:
-    32 * (2 C 2^k + (C + 3) 2^extended_k) resident, 32 * (2 C + 3) 2^k lean."""
+    32 * (2 C 2^k + (C + 3) 2^extended_k) resident, 32 * (2 C + 3) 2^k lean (on_demand and per_part)."""
     _check_cosets_mode(cosets)
     cols = cs.num_fixed + len(cs.permutation)
     if cosets == "resident":
@@ -456,11 +477,13 @@ def build_sigma(E, cs, k, copies):
 def keygen(E, cs, k, fixed_columns, copies, vk_digest=None, cosets="resident"):
     """keygen_vk + keygen_pk: fixed and sigma commitments, their coefficient forms and extended cosets, l0 / l_last /
     l_active cosets -- all left resident on the device. fixed_columns: list of (n, 4) Montgomery arrays (Lagrange).
-    cosets="on_demand" makes a lean key: no coset is ever computed, create_proof rebuilds them for each proof."""
+    cosets="on_demand" makes a lean key: no coset is ever computed, create_proof rebuilds them for each proof.
+    cosets="per_part" makes the same lean key, whose proofs build the cosets one n-row part at a time."""
     _check_cosets_mode(cosets)
     n = 1 << k
     pk = ProvingKey()
     pk.cs, pk.k, pk.n = cs, k, n
+    pk.per_part = cosets == "per_part"
     bf = cs.blinding_factors()
     pk.blinding_factors, pk.usable_rows = bf, n - (bf + 1)
     pk.fixed_values = [E.upload(c) for c in fixed_columns]
@@ -557,10 +580,11 @@ def write_pk(E, pk, path):
 def read_pk(E, cs, path, vk_digest=None, cosets="resident"):
     """ProvingKey::read: the inverse of write_pk; `cs` plays the role of the concrete circuit's configure().
     cosets="on_demand" reads a lean key from the same file: the coset sections are skipped, never read, and the three l
-    polynomials are rebuilt from their definition."""
+    polynomials are rebuilt from their definition. cosets="per_part" reads the same lean key for per-part proofs."""
     _check_cosets_mode(cosets)
-    lean = cosets == "on_demand"
+    lean = cosets != "resident"
     pk = ProvingKey()
+    pk.per_part = cosets == "per_part"
     with open(path, "rb") as f:
         head = f.read(8)
         k, n_fixed = int.from_bytes(head[:4], "big"), int.from_bytes(head[4:], "big")
@@ -629,6 +653,58 @@ def rotation_sets(queries_):
 
 
 # ---- create_proof -------------------------------------------------------------------------------------------------
+def evaluate_h_per_part(E, pk, advice_polys, inst_polys, perm_polys, lookups, beta, gamma, theta, y, lap):
+    """Evaluator::evaluate_h one coset part at a time (a per-part key); returns the extended `values` (2^extended_k rows).
+    Part j < R = 2^(extended_k - k) is the extended rows j + R m, m < n: the values at g_j omega^m with g_j = zeta
+    extended_omega^j. A rotation by r reads row (m + r) mod n of the same part, so the gate, permutation and lookup passes run
+    on a part with size n and rot_scale 1; only the permutation argument, which reads X itself, takes g_j. Every extended row
+    sees the same field operations in the same order as in the whole-coset evaluation, so `values` is the same.
+    Every part buffer is allocated once per proof and freed when this returns, before divide_by_vanishing."""
+    cs, k, n = pk.cs, pk.k, pk.n
+    R = 1 << (E.extended_k - k)
+    bf = pk.blinding_factors
+    ext_omega = pow(ROOT_OF_UNITY, 1 << (28 - E.extended_k), R_MOD)
+    omega = fr_mont(omega_of(k))
+    srcs = pk.fixed_polys + pk.sigma_polys + pk.l_polys + advice_polys + inst_polys + perm_polys
+    for L in lookups:
+        srcs += [L.product_poly, L.permuted_input_poly, L.permuted_table_poly]
+    parts = [E.alloc(n) for _ in srcs]
+    at = [0]
+
+    def take(count):
+        at[0] += count
+        return parts[at[0] - count:at[0]]
+    fixed_p, sigma_p, (l0, l_last, l_active) = take(len(pk.fixed_polys)), take(len(pk.sigma_polys)), take(3)
+    advice_p, inst_p, z_p = take(len(advice_polys)), take(len(inst_polys)), take(len(perm_polys))
+    lookup_p = [take(3) for _ in lookups]
+    cols = [{"fixed": fixed_p, "advice": advice_p, "instance": inst_p}[kind][c] for kind, c in cs.permutation]
+    gates = cs.gates_program() if cs.gates else None
+    table_programs = [cs.lookup_value_program(li) for li in range(len(lookups))]
+    part_values = E.alloc(n)
+    table_value = E.alloc(n) if lookups else None
+    values = E.alloc(1 << E.extended_k)
+    zero4 = fr_mont(0)
+    for j in range(R):
+        E.coeff_to_extended_part_many(srcs, j, parts)
+        lap("coeff_to_extended")
+        if j:
+            E.zero(part_values)                              # PreviousValue of the gates reads it: every part starts at zero
+        if gates is not None:
+            E.graph_evaluate(gates, fixed_p, advice_p, inst_p, beta, gamma, theta, y, part_values, n, 1)
+        if perm_polys:
+            g = fr_mont(ZETA * pow(ext_omega, j, R_MOD))
+            E.permutation_constraints(part_values, n, 1, -(bf + 1), cs.chunk_len(), z_p, cols, sigma_p, l0, l_last, l_active, beta, gamma, y, omega,
+                                      coset_generator=g)
+        for li, (pc, ic, tc) in enumerate(lookup_p):
+            if j or li:
+                E.zero(table_value)
+            E.graph_evaluate(table_programs[li], fixed_p, advice_p, inst_p, beta, gamma, theta, zero4, table_value, n, 1)
+            E.lookup_constraints(part_values, n, 1, pc, ic, tc, table_value, l0, l_last, l_active, beta, gamma, y)
+        E.extended_part_scatter(part_values, j, values)
+        lap("evaluate_h")
+    return values
+
+
 def create_proof(E, pk, instances, advice_columns, rng, transcript, timings=None):
     """halo2_proofs::plonk::create_proof for one circuit over KZG/SHPLONK (single phase, no challenges API).
     instances: per instance column a list of ints; advice_columns: per advice column an (n, 4) Montgomery array whose
@@ -743,36 +819,40 @@ def create_proof(E, pk, instances, advice_columns, rng, transcript, timings=None
     y = fr_mont(transcript.squeeze_challenge())
 
     # 7. quotient: extended cosets, evaluate_h, divide by the vanishing polynomial, split, commit
-    # a lean key's cosets are rebuilt here and freed with the advice cosets, before divide_by_vanishing
-    if pk.lean:
-        nf, ns = len(pk.fixed_polys), len(pk.sigma_polys)
-        key = coeff_to_extended_many(E, pk.fixed_polys + pk.sigma_polys + pk.l_polys)
-        fixed_cosets, sigma_cosets, (l0, l_last, l_active) = key[:nf], key[nf:nf + ns], key[nf + ns:]
-        del key
-        lap("key_cosets")
+    # a lean key's cosets are rebuilt here and freed with the advice cosets, before divide_by_vanishing; a per-part key's
+    # proof builds every coset one n-row part at a time (evaluate_h_per_part)
+    if pk.per_part:
+        values = evaluate_h_per_part(E, pk, advice_polys, inst_polys, perm_polys, lookups, beta, gamma, theta, y, lap)
     else:
-        fixed_cosets, sigma_cosets, l0, l_last, l_active = pk.fixed_cosets, pk.sigma_cosets, pk.l0, pk.l_last, pk.l_active
-    both = coeff_to_extended_many(E, advice_polys + inst_polys)
-    advice_cosets, inst_cosets = both[:len(advice_polys)], both[len(advice_polys):]
-    del both
-    lap("coeff_to_extended")
-    values = E.alloc(ext_n)
-    if cs.gates:
-        E.graph_evaluate(cs.gates_program(), fixed_cosets, advice_cosets, inst_cosets, beta, gamma, theta, y, values, ext_n, rot_scale)
-    if perm_polys:
-        z_cosets = coeff_to_extended_many(E, perm_polys)
-        cosets = [{"fixed": fixed_cosets, "advice": advice_cosets, "instance": inst_cosets}[kind][c] for kind, c in cs.permutation]
-        ext_omega = fr_mont(pow(ROOT_OF_UNITY, 1 << (28 - E.extended_k), R_MOD))
-        E.permutation_constraints(values, ext_n, rot_scale, -(bf + 1), chunk, z_cosets, cosets, sigma_cosets, l0, l_last, l_active, beta, gamma, y, ext_omega)
-        del z_cosets, cosets
-    for li, L in enumerate(lookups):
-        table_value = E.alloc(ext_n)
-        E.graph_evaluate(cs.lookup_value_program(li), fixed_cosets, advice_cosets, inst_cosets, beta, gamma, theta, zero4, table_value, ext_n, rot_scale)
-        pc, ic, tc = coeff_to_extended_many(E, [L.product_poly, L.permuted_input_poly, L.permuted_table_poly])
-        E.lookup_constraints(values, ext_n, rot_scale, pc, ic, tc, table_value, l0, l_last, l_active, beta, gamma, y)
-        del table_value, pc, ic, tc
-    del advice_cosets, inst_cosets, fixed_cosets, sigma_cosets, l0, l_last, l_active
-    lap("evaluate_h")
+        if pk.lean:
+            nf, ns = len(pk.fixed_polys), len(pk.sigma_polys)
+            key = coeff_to_extended_many(E, pk.fixed_polys + pk.sigma_polys + pk.l_polys)
+            fixed_cosets, sigma_cosets, (l0, l_last, l_active) = key[:nf], key[nf:nf + ns], key[nf + ns:]
+            del key
+            lap("key_cosets")
+        else:
+            fixed_cosets, sigma_cosets, l0, l_last, l_active = pk.fixed_cosets, pk.sigma_cosets, pk.l0, pk.l_last, pk.l_active
+        both = coeff_to_extended_many(E, advice_polys + inst_polys)
+        advice_cosets, inst_cosets = both[:len(advice_polys)], both[len(advice_polys):]
+        del both
+        lap("coeff_to_extended")
+        values = E.alloc(ext_n)
+        if cs.gates:
+            E.graph_evaluate(cs.gates_program(), fixed_cosets, advice_cosets, inst_cosets, beta, gamma, theta, y, values, ext_n, rot_scale)
+        if perm_polys:
+            z_cosets = coeff_to_extended_many(E, perm_polys)
+            cosets = [{"fixed": fixed_cosets, "advice": advice_cosets, "instance": inst_cosets}[kind][c] for kind, c in cs.permutation]
+            ext_omega = fr_mont(pow(ROOT_OF_UNITY, 1 << (28 - E.extended_k), R_MOD))
+            E.permutation_constraints(values, ext_n, rot_scale, -(bf + 1), chunk, z_cosets, cosets, sigma_cosets, l0, l_last, l_active, beta, gamma, y, ext_omega)
+            del z_cosets, cosets
+        for li, L in enumerate(lookups):
+            table_value = E.alloc(ext_n)
+            E.graph_evaluate(cs.lookup_value_program(li), fixed_cosets, advice_cosets, inst_cosets, beta, gamma, theta, zero4, table_value, ext_n, rot_scale)
+            pc, ic, tc = coeff_to_extended_many(E, [L.product_poly, L.permuted_input_poly, L.permuted_table_poly])
+            E.lookup_constraints(values, ext_n, rot_scale, pc, ic, tc, table_value, l0, l_last, l_active, beta, gamma, y)
+            del table_value, pc, ic, tc
+        del advice_cosets, inst_cosets, fixed_cosets, sigma_cosets, l0, l_last, l_active
+        lap("evaluate_h")
     E.divide_by_vanishing(values)
     pieces_n = cs.degree() - 1
     h_coeff = E.extended_to_coeff(values, n * pieces_n)

@@ -13,7 +13,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 def build_main_against_the_real_library(out_dir=None, main="prover_main"):
     """g++ tests/cpp/<main>.cpp -DSPB_PROVER_WITH_CUDART against libspectre_b200.so + cudart -> <out_dir>/<main>_cuda
     (default out_dir: a new temporary directory -- the checkout may be read-only). main="prover_main_lean" proves with a
-    lean key (cosets rebuilt per proof)."""
+    lean key (cosets rebuilt per proof), main="prover_main_per_part" with a per-part key (the quotient one coset part at a time)."""
     from spectre_b200 import build
     lib = build.build()
     libdir = os.path.dirname(lib)

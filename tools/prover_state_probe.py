@@ -1,19 +1,21 @@
 #!/usr/bin/env python3
-"""What lean proving keys (cosets="on_demand") buy a process that holds Spectre's four proving keys on one device, as
-ProverState::new does (sync-step and committee-update at k = 20, their aggregations at K = 23 and K = 24).
+"""What lean proving keys (cosets="on_demand") and per-part keys (cosets="per_part") buy a process that holds Spectre's four
+proving keys on one device, as ProverState::new does (sync-step and committee-update at k = 20, their aggregations at K = 23
+and K = 24).
 
     python tools/prover_state_probe.py [--keys sync_step_shape:20,aggregation_shape:23,aggregation_shape:24] [--reps 3] [--no-four-keys] [--out FILE]
 
-Per key shape, for both residency modes, on the first GPU:
+Per key shape, for every residency mode, on the first GPU:
   * the device bytes the key holds after keygen, from torch.cuda.mem_get_info (which also sees the library's own cudaMallocs;
     the library's workspaces are released before both readings), next to plonk.key_device_bytes and to the change of
     torch.cuda.memory_allocated. mem_get_info counts the whole device, so on a device shared with other processes, and at
     small k where the allocator's 2 MiB segments dominate, it can differ from the other two;
-  * create_proof wall time, best of `reps` warm runs after one warm-up run, and whether both modes give the same proof bytes.
-Then the four-key run: all four keys loaded lean, params at k = 20, 23 and 24 with the default window tables, then one proof per
+  * create_proof wall time, best of `reps` warm runs after one warm-up run, and whether every mode gives the same proof bytes.
+Then the four-key run: the three smaller keys loaded lean (on_demand) and the K = 24 key per_part (or on_demand with
+--k24-cosets on_demand), params at k = 20, 23 and 24 with the default window tables, then one proof per
 key in turn, each after the library's workspaces are released. It records the free device memory after each load and before
-each proof, the lowest free memory seen at each create_proof stage lap (the `timings` hook), and whether each proof, the K = 24
-one last, completed. If the K = 24 proof does not fit, it is repeated with only its own key and params loaded, and the
+each proof, the lowest free memory seen at each create_proof stage lap (the `timings` hook), each stage's time, and whether
+each proof, the K = 24 one last, completed. If the K = 24 proof does not fit, it is repeated with only its own key and params loaded, and the
 shortfall is its working set there minus the memory the four-key state left free. The committee-update k = 20 key uses the
 sync-step shape as a stand-in. Witnesses and RNG are bench.py's. Prints one JSON document (and writes it to --out).
 """
@@ -81,17 +83,18 @@ def per_key(torch, be, name, k, reps):
                      "keygen_s": round(t_keygen, 3), "create_proof_s": round(min(runs[1:]), 4), "warm_runs_s": [round(t, 4) for t in runs[1:]],
                      "first_run_s": round(runs[0], 4)}
         del pk
-    row["proofs_equal"] = proofs["resident"] == proofs["on_demand"]
+    row["proofs_equal"] = all(p == proofs["resident"] for p in proofs.values())
     row["lean_extra_s"] = round(row["on_demand"]["create_proof_s"] - row["resident"]["create_proof_s"], 4)
+    row["per_part_extra_s"] = round(row["per_part"]["create_proof_s"] - row["resident"]["create_proof_s"], 4)
     row["held_saved_share"] = round(1 - row["on_demand"]["held_bytes"] / row["resident"]["held_bytes"], 3)
     del E, params
     free_bytes(torch, 0)
     return row
 
 
-def four_keys(torch, be):
+def four_keys(torch, be, k24_cosets):
     dev = torch.device("cuda", be.devices[0])
-    out = {"free_at_start_gib": round(free_bytes(torch, dev) / GIB, 3)}
+    out = {"k24_cosets": k24_cosets, "free_at_start_gib": round(free_bytes(torch, dev) / GIB, 3)}
     params = {k: halo2.ParamsKZG.setup(be, k, SECRET).precompute() for k in (20, 23, 24)}
     out["free_after_params_gib"] = round(free_bytes(torch, dev) / GIB, 3)
     keys = []
@@ -99,7 +102,7 @@ def four_keys(torch, be):
                            ("sync_step_aggregation", "aggregation_shape", 23), ("committee_update_aggregation", "aggregation_shape", 24)):
         cs, inst, fixed, _, pinned, copies, _ = make_case(torch, name, k)
         E = plonk.DeviceEngine(be, params[k], k, cs.degree())
-        pk = plonk.keygen(E, cs, k, fixed, copies, vk_digest=BENCH_VK_DIGEST, cosets="on_demand")
+        pk = plonk.keygen(E, cs, k, fixed, copies, vk_digest=BENCH_VK_DIGEST, cosets=k24_cosets if k == 24 else "on_demand")
         del fixed
         be.release_workspace()
         keys.append((label, E, pk, inst, pinned))
@@ -131,6 +134,7 @@ def proof_with_laps(torch, be, dev, E, pk, inst, pinned):
     except Exception as e:                                     # out of device memory: record how far it got
         rec.update(completed=False, error=repr(e)[:300])
     rec["lowest_free_gib_at_lap"] = {name: round(v / GIB, 3) for name, v in laps.low.items()}
+    rec["stage_s"] = {name: round(v, 4) for name, v in laps.items()}
     rec["lowest_free_gib"] = round(min(laps.low.values()) / GIB, 3) if laps.low else None
     free_bytes(torch, dev)
     return rec
@@ -141,19 +145,20 @@ def main():
     ap.add_argument("--keys", default="sync_step_shape:20,aggregation_shape:23,aggregation_shape:24")
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--no-four-keys", action="store_true")
+    ap.add_argument("--k24-cosets", default="per_part", choices=plonk.COSETS_MODES[1:], help="residency of the K = 24 key in the four-key run")
     ap.add_argument("--out")
     args = ap.parse_args()
     import torch
     be = halo2.Backend([0])
     name, watts = gpu_identity()
-    result = {"what": "proving-key residency: resident vs on_demand (lean) cosets", "gpu": name, "power_limit_w": watts,
+    result = {"what": "proving-key residency: resident vs on_demand (lean) vs per_part cosets", "gpu": name, "power_limit_w": watts,
               "device_total_gib": round(torch.cuda.mem_get_info(0)[1] / GIB, 3), "keys": []}
     for spec in filter(None, args.keys.split(",")):
         shape, k = spec.split(":")
         result["keys"].append(per_key(torch, be, shape, int(k), args.reps))
         print(json.dumps(result["keys"][-1]), file=sys.stderr, flush=True)
     if not args.no_four_keys:
-        result["four_keys_lean"] = four_keys(torch, be)
+        result["four_keys_lean"] = four_keys(torch, be, args.k24_cosets)
     be.close()
     text = json.dumps(result, indent=1)
     print(text)
