@@ -296,6 +296,30 @@ int spb_lookup_constraints_dev(spb_ctx* ctx, spb_fr* d_values, uint64_t size, in
  * Returns SPB_ERR_CONSTRAINT when an input value does not occur in the table. */
 int spb_permute_expression_pair_dev(spb_ctx* ctx, const spb_fr* d_input, const spb_fr* d_table, size_t usable, spb_fr* d_permuted_input, spb_fr* d_permuted_table);
 
+/* ---- witness check ([UPSTREAM] halo2_proofs/src/dev.rs, MockProver::verify) ------------------------------------------ */
+/* Each of the three reports the first `cap` failing rows in ascending order and the exact count of failing rows; only those
+ * cross PCIe. Inputs are device buffers of the context's first device and are not written; outputs are HOST arrays, filled
+ * before the call returns. A NULL context, or a NULL pointer the call would read or write, is SPB_ERR_ARG. A call with no
+ * rows to check launches nothing and reports 0.
+ * Kernel launches (spb_kernel_launches): spb_nonzero_rows_dev 2; spb_lookup_missing_rows_dev 12 + 2 per non-trivial digit
+ * pass of the table's radix sort (a pass runs for each byte of each 64-bit limb of the canonical values on which the usable
+ * table rows do not all agree); spb_copy_mismatches_dev 2 per column. */
+/* rows_out[0 .. min(cap, total)) = the rows r in [lo, hi) with d_values[r] != 0, ascending; *total_out = their number.
+ * hi must be below 2^32. Used on a gate evaluated over the n Lagrange rows. */
+int spb_nonzero_rows_dev(spb_ctx* ctx, const spb_fr* d_values, uint64_t lo, uint64_t hi, uint32_t cap, uint32_t* rows_out, uint64_t* total_out);
+/* Lookup membership: the rows r < usable whose d_input[r] equals no d_table[j], j < usable (both compressed with the same theta,
+ * Montgomery form); reported as spb_nonzero_rows_dev reports. The table's usable rows are sorted in the workspace of
+ * spb_permute_expression_pair_dev, so the check needs no more device memory than that call. */
+int spb_lookup_missing_rows_dev(spb_ctx* ctx, const spb_fr* d_input, const spb_fr* d_table, size_t usable, uint32_t cap, uint32_t* rows_out, uint64_t* total_out);
+/* Copy constraints of n_cols permutation columns over n = 2^k rows (HOST arrays of device pointers to their Lagrange values and
+ * sigma columns). For every column c and row i < usable, the cell (c', i') that sigma_c[i] = delta^c' omega^i' labels must hold
+ * the same value as (c, i). For column c, cells_out[4 (c cap + m) ..] = (c, i, c', i') of its m-th failing row, m < min(cap,
+ * totals_out[c]), and totals_out[c] = its number of failing rows. A sigma entry of a usable row that labels no cell of a
+ * usable row (c' >= n_cols or i' >= usable) is a malformed key: SPB_ERR_DATA, and the error text names the column and row
+ * of the first such entry (lowest column, then lowest row); the outputs are then only the zeroed totals. usable <= 2^k. */
+int spb_copy_mismatches_dev(spb_ctx* ctx, uint32_t k, const spb_fr* const* d_values, const spb_fr* const* d_sigma, uint32_t n_cols, size_t usable, uint32_t cap,
+                            uint32_t* cells_out, uint64_t* totals_out);
+
 /* ---- argument provers, device resident ([UPSTREAM] halo2_proofs/src/plonk/{permutation,lookup}/prover.rs) ----------- */
 /* permutation::Argument::commit for ONE set (a chunk of <= degree-2 columns, first_col = its index of first column in
  * the permutation): over all n = 2^k rows

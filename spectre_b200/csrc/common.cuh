@@ -191,6 +191,21 @@ int dev_batch_invert(spb_ctx* ctx, DeviceState& d, Fr* da, size_t n);
 int dev_product_enqueue(spb_ctx* ctx, DeviceState& d, const Fr* da, size_t n, Fr** d_total);  // *d_total: one Fr on device d, valid after the enqueued work
 int dev_eval_polynomial(spb_ctx* ctx, DeviceState& d, const Fr* dp, size_t n, const Fr& x, Fr* out_host);  // synchronises
 
+// ---- lookup.cu: the workspace of permute_expression_pair over n rows (context slots "lk_*") and its canonical sort ----
+struct LookupWork {
+  Fr *canon, *sin, *stb;                        // n each
+  uint32_t *idx_a, *idx_b;                      // n each
+  unsigned long long *keys_a, *keys_b;          // n each
+  uint32_t* flags;                              // 4 n + 8
+  int* err;
+  uint32_t *rs_hist, *rs_tile;                  // radix-sort histograms
+  void* tmp; size_t tmp_bytes;                  // cub scan temp, enough for n + 1 u32
+};
+int lookup_work(spb_ctx* ctx, DeviceState& d, uint64_t n, LookupWork* w);
+// sorted[i] = the canonical values of src's n rows in ascending order (w.canon, w.idx_*, w.keys_* and the histograms are
+// overwritten; sorted may be w.sin or w.stb)
+int sort_canonical(spb_ctx* ctx, DeviceState& d, const LookupWork& w, const Fr* src, Fr* sorted, uint64_t n);
+
 // ---- host field helpers (64-bit path) ----
 inline Fr fr_from_u64(uint64_t v) {
   Fr a = fp_zero<FrParams>(); a.l[0] = (uint32_t)v; a.l[1] = (uint32_t)(v >> 32);

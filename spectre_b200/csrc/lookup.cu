@@ -171,18 +171,39 @@ __global__ void lk_emit_leftover_kernel(const Fr* stb, const uint32_t* left_flag
   ntt_stg(ptab + rep_rows[m - 1 - r], fp_to_mont(ntt_ldg(stb + j)));
 }
 
-namespace {
-// sorted[i] = canonical values of src in ascending order (idx/keys/scratch are n-sized work arrays)
-int sort_canonical(spb_ctx* ctx, DeviceState& d, const Fr* src, Fr* canon, Fr* sorted, uint32_t* idx_a, uint32_t* idx_b, unsigned long long* keys_a,
-                   unsigned long long* keys_b, uint32_t* hist, uint32_t* tile_hist, void* tmp, size_t tmp_bytes, uint64_t n) {
-  SPB_TRY(launch(ctx, d.stream, nblk(n, 256), 256, 0, lk_canon_kernel, src, canon, idx_a, n));
-  for (uint32_t limb = 0; limb < 4; limb++) {
-    SPB_TRY(launch(ctx, d.stream, nblk(n, 256), 256, 0, lk_gather_limb_kernel, canon, idx_a, limb, keys_a, n));
-    SPB_TRY(radix_sort_pairs_u64(ctx, d, keys_a, keys_b, idx_a, idx_b, n, hist, tile_hist, tmp, tmp_bytes));   // result back in keys_a / idx_a
-  }
-  return launch(ctx, d.stream, nblk(n, 256), 256, 0, lk_gather_kernel, canon, idx_a, sorted, n);
+namespace spb {
+int lookup_work(spb_ctx* ctx, DeviceState& d, uint64_t n, LookupWork* w) {
+  w->canon = (Fr*)slot(ctx, d, "lk_canon", n * 32);
+  w->sin = (Fr*)slot(ctx, d, "lk_sin", n * 32);
+  w->stb = (Fr*)slot(ctx, d, "lk_stb", n * 32);
+  w->idx_a = (uint32_t*)slot(ctx, d, "lk_idx_a", n * 4);
+  w->idx_b = (uint32_t*)slot(ctx, d, "lk_idx_b", n * 4);
+  w->keys_a = (unsigned long long*)slot(ctx, d, "lk_keys_a", n * 8);
+  w->keys_b = (unsigned long long*)slot(ctx, d, "lk_keys_b", n * 8);
+  w->flags = (uint32_t*)slot(ctx, d, "lk_flags", (4 * n + 8) * 4);   // permute_expression_pair: repeated_flag | rep_rank | used->left_flag | left_rank
+  w->err = (int*)slot(ctx, d, "lk_err", 16);
+  const uint32_t ntiles = (uint32_t)((n + kRsTile - 1) / kRsTile);
+  w->rs_hist = (uint32_t*)slot(ctx, d, "lk_rs_hist", 8 * 256 * 4);
+  w->rs_tile = (uint32_t*)slot(ctx, d, "lk_rs_tile", ((size_t)256 * ntiles + 1) * 4);
+  size_t scan_a = 0, scan_b = 0;
+  cub::DeviceScan::ExclusiveSum(nullptr, scan_a, w->flags, w->flags, (int)n + 1, d.stream);
+  cub::DeviceScan::ExclusiveSum(nullptr, scan_b, w->rs_tile, w->rs_tile, (int)(256 * ntiles), d.stream);
+  w->tmp_bytes = scan_a > scan_b ? scan_a : scan_b;
+  w->tmp = slot(ctx, d, "lk_tmp", w->tmp_bytes ? w->tmp_bytes : 16);
+  if (!w->canon || !w->sin || !w->stb || !w->idx_a || !w->idx_b || !w->keys_a || !w->keys_b || !w->flags || !w->err || !w->tmp || !w->rs_hist || !w->rs_tile)
+    return SPB_ERR_OOM;
+  return 0;
 }
-}  // namespace
+
+int sort_canonical(spb_ctx* ctx, DeviceState& d, const LookupWork& w, const Fr* src, Fr* sorted, uint64_t n) {
+  SPB_TRY(launch(ctx, d.stream, nblk(n, 256), 256, 0, lk_canon_kernel, src, w.canon, w.idx_a, n));
+  for (uint32_t limb = 0; limb < 4; limb++) {
+    SPB_TRY(launch(ctx, d.stream, nblk(n, 256), 256, 0, lk_gather_limb_kernel, w.canon, w.idx_a, limb, w.keys_a, n));
+    SPB_TRY(radix_sort_pairs_u64(ctx, d, w.keys_a, w.keys_b, w.idx_a, w.idx_b, n, w.rs_hist, w.rs_tile, w.tmp, w.tmp_bytes));   // result back in keys_a / idx_a
+  }
+  return launch(ctx, d.stream, nblk(n, 256), 256, 0, lk_gather_kernel, w.canon, w.idx_a, sorted, n);
+}
+}  // namespace spb
 
 extern "C" {
 
@@ -192,28 +213,17 @@ int spb_permute_expression_pair_dev(spb_ctx* ctx, const spb_fr* d_input, const s
   if (usable >= 0x7fffffffull) return SPB_ERR_ARG;
   SPB_ENTER(ctx);
   const uint64_t n = usable;
-  Fr* canon = (Fr*)slot(ctx, d, "lk_canon", n * 32);
-  Fr* sin = (Fr*)slot(ctx, d, "lk_sin", n * 32);
-  Fr* stb = (Fr*)slot(ctx, d, "lk_stb", n * 32);
-  uint32_t* idx_a = (uint32_t*)slot(ctx, d, "lk_idx_a", n * 4);
-  uint32_t* idx_b = (uint32_t*)slot(ctx, d, "lk_idx_b", n * 4);
-  unsigned long long* keys_a = (unsigned long long*)slot(ctx, d, "lk_keys_a", n * 8);
-  unsigned long long* keys_b = (unsigned long long*)slot(ctx, d, "lk_keys_b", n * 8);
-  uint32_t* flags = (uint32_t*)slot(ctx, d, "lk_flags", (4 * n + 8) * 4);   // repeated_flag | rep_rank | used->left_flag | left_rank
-  int* err = (int*)slot(ctx, d, "lk_err", 16);
-  const uint32_t ntiles = (uint32_t)((n + kRsTile - 1) / kRsTile);
-  uint32_t* rs_hist = (uint32_t*)slot(ctx, d, "lk_rs_hist", 8 * 256 * 4);
-  uint32_t* rs_tile = (uint32_t*)slot(ctx, d, "lk_rs_tile", ((size_t)256 * ntiles + 1) * 4);
-  size_t scan_a = 0, scan_b = 0;
-  cub::DeviceScan::ExclusiveSum(nullptr, scan_a, flags, flags, (int)n + 1, d.stream);
-  cub::DeviceScan::ExclusiveSum(nullptr, scan_b, rs_tile, rs_tile, (int)(256 * ntiles), d.stream);
-  size_t tmp_bytes = scan_a > scan_b ? scan_a : scan_b;
-  void* tmp = slot(ctx, d, "lk_tmp", tmp_bytes ? tmp_bytes : 16);
-  if (!canon || !sin || !stb || !idx_a || !idx_b || !keys_a || !keys_b || !flags || !err || !tmp || !rs_hist || !rs_tile) return SPB_ERR_OOM;
-  uint32_t* repeated_flag = flags, *rep_rank = flags + (n + 1), *used = flags + 2 * (n + 1), *left_rank = flags + 3 * (n + 1);
+  LookupWork w;
+  SPB_TRY(lookup_work(ctx, d, n, &w));
+  Fr* sin = w.sin, *stb = w.stb;
+  uint32_t* flags = w.flags, *used = flags + 2 * (n + 1);
+  void* tmp = w.tmp;
+  size_t tmp_bytes = w.tmp_bytes;
+  int* err = w.err;
+  uint32_t* repeated_flag = flags, *rep_rank = flags + (n + 1), *left_rank = flags + 3 * (n + 1);
 
-  SPB_TRY(sort_canonical(ctx, d, (const Fr*)d_input, canon, sin, idx_a, idx_b, keys_a, keys_b, rs_hist, rs_tile, tmp, tmp_bytes, n));
-  SPB_TRY(sort_canonical(ctx, d, (const Fr*)d_table, canon, stb, idx_a, idx_b, keys_a, keys_b, rs_hist, rs_tile, tmp, tmp_bytes, n));
+  SPB_TRY(sort_canonical(ctx, d, w, (const Fr*)d_input, sin, n));
+  SPB_TRY(sort_canonical(ctx, d, w, (const Fr*)d_table, stb, n));
   SPB_CUDA(ctx, cudaMemsetAsync(flags, 0, (4 * n + 8) * 4, d.stream));
   SPB_CUDA(ctx, cudaMemsetAsync(err, 0, 4, d.stream));
   SPB_TRY(launch(ctx, d.stream, nblk(n, 256), 256, 0, lk_match_kernel, sin, stb, n, repeated_flag, used, err));
@@ -226,7 +236,7 @@ int spb_permute_expression_pair_dev(spb_ctx* ctx, const spb_fr* d_input, const s
   SPB_CUDA(ctx, cudaMemcpyAsync(&herr, err, 4, cudaMemcpyDeviceToHost, d.stream));
   SPB_CUDA(ctx, cudaStreamSynchronize(d.stream));
   if (herr || counts[0] != counts[1]) return set_error(ctx, SPB_ERR_CONSTRAINT, "permute_expression_pair: an input value does not occur in the table (ConstraintSystemFailure)");
-  uint32_t* rep_rows = idx_b;   // free again
+  uint32_t* rep_rows = w.idx_b;   // free again
   SPB_TRY(launch(ctx, d.stream, nblk(n, 256), 256, 0, lk_emit_input_kernel, sin, repeated_flag, rep_rank, rep_rows, (Fr*)d_permuted_input, (Fr*)d_permuted_table, n));
   SPB_TRY(launch(ctx, d.stream, nblk(n, 256), 256, 0, lk_emit_leftover_kernel, stb, used, left_rank, rep_rows, counts[0], (Fr*)d_permuted_table, n));
   SPB_CUDA(ctx, cudaStreamSynchronize(d.stream));

@@ -347,6 +347,35 @@ class Backend:
         self.check(self.lib.spb_permute_expression_pair_dev(self.ctx, _p(d_input), _p(d_table), ctypes.c_size_t(usable), _p(d_permuted_input),
                                                             _p(d_permuted_table)), "spb_permute_expression_pair_dev")
 
+    # ---- witness check (dev::MockProver::verify) ----------------------------------------------------------
+    def nonzero_rows_dev(self, d_values, lo, hi, cap):
+        """-> (the first `cap` rows r in [lo, hi) with values[r] != 0, ascending; their total number)"""
+        rows, total = np.zeros(max(cap, 1), dtype=np.uint32), ctypes.c_uint64()
+        self.check(self.lib.spb_nonzero_rows_dev(self.ctx, _p(d_values), ctypes.c_uint64(lo), ctypes.c_uint64(hi), ctypes.c_uint32(cap), _p(rows),
+                                                 ctypes.byref(total)), "spb_nonzero_rows_dev")
+        return [int(r) for r in rows[:min(cap, total.value)]], total.value
+
+    def lookup_missing_rows_dev(self, d_input, d_table, usable, cap):
+        """-> (the first `cap` rows r < usable whose input value is not among the table's usable rows, ascending; their total number)"""
+        rows, total = np.zeros(max(cap, 1), dtype=np.uint32), ctypes.c_uint64()
+        self.check(self.lib.spb_lookup_missing_rows_dev(self.ctx, _p(d_input), _p(d_table), ctypes.c_size_t(usable), ctypes.c_uint32(cap), _p(rows),
+                                                        ctypes.byref(total)), "spb_lookup_missing_rows_dev")
+        return [int(r) for r in rows[:min(cap, total.value)]], total.value
+
+    def copy_mismatches_dev(self, k, d_values, d_sigma, usable, cap):
+        """-> per permutation column: (its total of failing rows, [(row, col', row') of the first `cap`, ascending]).
+        A sigma entry that labels no usable cell raises with ERR_DATA's text naming its column and row."""
+        m = len(d_values)
+        mk = lambda ps: (ctypes.c_void_p * max(1, len(ps)))(*ps)
+        cells, totals = np.zeros((max(m * cap, 1), 4), dtype=np.uint32), np.zeros(max(m, 1), dtype=np.uint64)
+        self.check(self.lib.spb_copy_mismatches_dev(self.ctx, ctypes.c_uint32(k), mk(d_values), mk(d_sigma), ctypes.c_uint32(m), ctypes.c_size_t(usable),
+                                                    ctypes.c_uint32(cap), _p(cells), _p(totals)), "spb_copy_mismatches_dev")
+        out = []
+        for c in range(m):
+            t = int(totals[c])
+            out.append((t, [(int(r), int(c2), int(r2)) for _, r, c2, r2 in cells[c * cap:c * cap + min(cap, t)]]))
+        return out
+
     # ---- file <-> device streaming (params / proving-key files) -------------------------------------------
     def read_file_dev(self, path, offset, d_dst, nbytes):
         self.check(self.lib.spb_read_file_dev(self.ctx, path.encode(), ctypes.c_uint64(offset), _p(d_dst), ctypes.c_size_t(nbytes)), "spb_read_file_dev")

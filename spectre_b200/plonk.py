@@ -17,6 +17,9 @@ parity tests bind the same driver to the CPU oracle and require byte-identical p
 A circuit is described by a `ConstraintSystem` of expression trees -- the information `pk.get_vk().cs()` holds
 upstream. Expressions are nested tuples built with Const / Fixed / Advice / Instance / Neg / Sum / Prod / Scaled.
 """
+import secrets
+from collections import namedtuple
+
 import numpy as np
 
 from . import halo2
@@ -349,6 +352,12 @@ class DeviceEngine:
         return self.be.permutation_product_dev(self.k, [b.data_ptr() for b in values], [b.data_ptr() for b in sigma], first_col, beta, gamma, blinds, last_z, z.data_ptr())
     def lookup_product(self, ci, ct, pi, pt, beta, gamma, blinds, z):
         self.be.lookup_product_dev(self.n, ci.data_ptr(), ct.data_ptr(), pi.data_ptr(), pt.data_ptr(), beta, gamma, blinds, z.data_ptr())
+
+    # witness check
+    def nonzero_rows(self, values, lo, hi, cap): return self.be.nonzero_rows_dev(values.data_ptr(), lo, hi, cap)
+    def lookup_missing_rows(self, ci, ct, usable, cap): return self.be.lookup_missing_rows_dev(ci.data_ptr(), ct.data_ptr(), usable, cap)
+    def copy_mismatches(self, values, sigma, usable, cap):
+        return self.be.copy_mismatches_dev(self.k, [b.data_ptr() for b in values], [b.data_ptr() for b in sigma], usable, cap)
 
     # batch ops
     def eval_polynomial(self, b, n, point): return self.be.eval_polynomial_dev(b.data_ptr(), n, point)
@@ -927,3 +936,62 @@ def create_proof(E, pk, instances, advice_columns, rng, transcript, timings=None
     transcript.write_ec_point(E.shplonk_finish(state, u))
     lap("shplonk")
     return bytes(transcript.proof)
+
+
+# ---- witness check ------------------------------------------------------------------------------------------------
+class WitnessFailure(namedtuple("WitnessFailure", "kind index rows total mapped", defaults=(None,))):
+    """One failing constraint of check_witness. kind: "gate" (index = the gate's position in cs.gates), "lookup" (its
+    position in cs.lookups) or "copy" (the permutation column's position in cs.permutation); rows: the first failing rows,
+    ascending; total: how many rows fail; mapped: for "copy", the (column, row) each of `rows` is copied to (else None)."""
+
+
+def check_witness(E, pk, instances, advice_columns, theta=None, max_rows=16):
+    """halo2_proofs::dev::MockProver::verify on the engine: every constraint the witness fails, as a list of WitnessFailure in
+    the order gates, lookups, permutation columns; [] for a satisfied witness. Nothing is written to the key, and the
+    caller's columns are uploaded as they are (no blinding rows are drawn), so it can run before or instead of create_proof.
+
+    With u = pk.usable_rows and n = 2^k, every read is of the n-row Lagrange values, rotations wrapping mod n:
+      * a gate must evaluate to zero at every row i < u (a rotated read into the rows >= u reads what the caller put there);
+      * a lookup's input tuple at every row i < u must equal its table tuple at some row j < u. Both sides are compressed with
+        a random theta as create_proof compresses them (theta=None draws it from `secrets`); a tuple that is in no table row
+        passes only if its compression collides with one of the u table values, probability about u / r for the field size r;
+      * at every row i < u of permutation column c, the cell must hold the value of the cell (c', i') that sigma_c[i] labels.
+    Instances are laid out as create_proof lays them out. A key whose sigma labels a cell outside the usable rows raises the
+    engine's error naming the column and row."""
+    cs, n, usable = pk.cs, pk.n, pk.usable_rows
+    if len(instances) != cs.num_instance:
+        raise ValueError("check_witness: %d instance columns given, the circuit has %d (upstream: Error::InvalidInstances)" % (len(instances), cs.num_instance))
+    if len(advice_columns) != cs.num_advice:
+        raise ValueError("check_witness: %d advice columns given, the circuit has %d" % (len(advice_columns), cs.num_advice))
+    inst_values = []
+    for col in instances:
+        if len(col) > usable:
+            raise ValueError("check_witness: an instance column has more than %d values (upstream: Error::InstanceTooLarge)" % usable)
+        b = E.alloc(n); E.write_rows(b, 0, fr_mont_rows(col)); inst_values.append(b)
+    advice_values = [E.upload(col) for col in advice_columns]
+    fixed = pk.fixed_values
+    zero4 = fr_mont(0)
+    failures = []
+    if cs.gates:
+        values = E.alloc(n)
+        for g, gate in enumerate(cs.gates):
+            p = Program()
+            p.horner(p._const(0), p._const(0), [gate])           # 0 * 0 + gate: this gate alone, no y-folding
+            E.graph_evaluate(p.finish(), fixed, advice_values, inst_values, zero4, zero4, zero4, zero4, values, n, 1)
+            rows, total = E.nonzero_rows(values, 0, usable, max_rows)
+            if total:
+                failures.append(WitnessFailure("gate", g, rows, total))
+    theta = fr_mont(secrets.randbelow(R_MOD) if theta is None else theta)
+    for li, (ins, tbs) in enumerate(cs.lookups):
+        ci, ct = E.alloc(n), E.alloc(n)
+        E.graph_evaluate(cs.lookup_compress_program(ins), fixed, advice_values, inst_values, zero4, zero4, theta, zero4, ci, n, 1)
+        E.graph_evaluate(cs.lookup_compress_program(tbs), fixed, advice_values, inst_values, zero4, zero4, theta, zero4, ct, n, 1)
+        rows, total = E.lookup_missing_rows(ci, ct, usable, max_rows)
+        if total:
+            failures.append(WitnessFailure("lookup", li, rows, total))
+    if cs.permutation:
+        cols = [{"fixed": fixed, "advice": advice_values, "instance": inst_values}[kind][c] for kind, c in cs.permutation]
+        for c, (total, cells) in enumerate(E.copy_mismatches(cols, pk.sigma_values, usable, max_rows)):
+            if total:
+                failures.append(WitnessFailure("copy", c, [r for r, _, _ in cells], total, [(c2, r2) for _, c2, r2 in cells]))
+    return failures
