@@ -320,6 +320,29 @@ int spb_lookup_missing_rows_dev(spb_ctx* ctx, const spb_fr* d_input, const spb_f
 int spb_copy_mismatches_dev(spb_ctx* ctx, uint32_t k, const spb_fr* const* d_values, const spb_fr* const* d_sigma, uint32_t n_cols, size_t usable, uint32_t cap,
                             uint32_t* cells_out, uint64_t* totals_out);
 
+/* ---- proving-key check ([UPSTREAM] halo2_proofs/src/plonk.rs ProvingKey::read in SerdeFormat::RawBytes, and
+ * permutation::keygen::Assembly) ---------------------------------------------------------------------------------------
+ * Inputs are device buffers of the context's first device and are not written; outputs are HOST values, filled before the call
+ * returns. A NULL context, or a NULL pointer the call would read or write, is SPB_ERR_ARG.
+ * Kernel launches (spb_kernel_launches): spb_fr_first_noncanonical_dev 1 (0 when n = 0); spb_sigma_check_dev 7 per column,
+ * less 2 per column when usable = 2^k (no blinding rows) and 2 per column when usable = 0 (0 when n_cols = 0). */
+/* *first_out = the lowest index i < n whose stored limbs, read as a 256-bit integer, are >= r (halo2curves' from_raw_bytes
+ * rejects them); n when every element is canonical. Used on each polynomial of a .pkey right after it lands in device memory. */
+int spb_fr_first_noncanonical_dev(spb_ctx* ctx, const spb_fr* d, size_t n, uint64_t* first_out);
+/* Is sigma (n_cols HOST-held device pointers, 2^k rows each) a permutation of the cells (c, i), c < n_cols, i < 2^k, of the kind
+ * permutation::keygen::Assembly builds? sigma_c[i] = delta^c' omega^i' labels the cell (c', i'). Three kinds of failure q, for
+ * each column c: totals_out[3 c + q] = their exact number, rows_out[(3 c + q) cap + m] = the m-th row, ascending, m < min(cap,
+ * total):
+ *   q = 0 (label):      rows i < usable whose sigma_c[i] labels no cell of a usable row (no column c' < n_cols, or i' >= usable);
+ *   q = 1 (blinding):   rows i >= usable whose sigma_c[i] is not their own label delta^c omega^i (Assembly::copy refuses rows
+ *                       >= usable, so they are fixed points);
+ *   q = 2 (unlabelled): cells (c, i), i < 2^k, that no sigma entry of any column labels.
+ * All totals zero: as many entries as cells, each labels a cell and every cell is labelled, so sigma is a bijection of the cells
+ * that fixes the blinding rows. Each entry is decoded once (a fixed point needs no decode) and its cell marked in an
+ * n_cols 2^k-bit map; the report does not depend on the order of the device's atomics. usable <= 2^k, k <= 28. */
+int spb_sigma_check_dev(spb_ctx* ctx, uint32_t k, const spb_fr* const* d_sigma, uint32_t n_cols, size_t usable, uint32_t cap, uint32_t* rows_out,
+                        uint64_t* totals_out);
+
 /* ---- argument provers, device resident ([UPSTREAM] halo2_proofs/src/plonk/{permutation,lookup}/prover.rs) ----------- */
 /* permutation::Argument::commit for ONE set (a chunk of <= degree-2 columns, first_col = its index of first column in
  * the permutation): over all n = 2^k rows

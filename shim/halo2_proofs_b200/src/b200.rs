@@ -150,6 +150,13 @@ extern "C" {
     ) -> c_int;
     pub fn spb_shplonk_finish_dev(ctx: *mut spb_ctx, s: *mut spb_shplonk, u: *const Fr, out: *mut G1) -> c_int;
     pub fn spb_shplonk_abort(ctx: *mut spb_ctx, s: *mut spb_shplonk);
+    // ---- proving-key check (ProvingKey::read in SerdeFormat::RawBytes; sigma as Assembly builds it) ----
+    /// `*first_out` = the first element of `d` whose stored limbs are not below r, or `n`
+    pub fn spb_fr_first_noncanonical_dev(ctx: *mut spb_ctx, d: *const Fr, n: usize, first_out: *mut u64) -> c_int;
+    /// per column c and kind q (0 label, 1 blinding, 2 unlabelled): `totals_out[3c + q]`, first rows at `rows_out[(3c + q) cap ..]`
+    pub fn spb_sigma_check_dev(
+        ctx: *mut spb_ctx, k: u32, d_sigma: *const *const Fr, n_cols: u32, usable: usize, cap: u32, rows_out: *mut u32, totals_out: *mut u64,
+    ) -> c_int;
 }
 
 /// The process-wide context. `SPECTRE_B200_GPUS=N` (default 1) makes it drive N devices: SRS bases are sharded by point

@@ -123,6 +123,22 @@ int launch(spb_ctx* ctx, cudaStream_t stream, dim3 grid, dim3 block, size_t smem
   return 0;
 }
 
+// Lowest index i < n with bad(i), folded into *first (all ones before the launch). Only a thread that finds a bad element
+// touches the atomic, and it stops there: its later indices are larger. The params check (msm.cu) and the proving-key check
+// (witness.cu) each pass their own predicate.
+template <class Bad>
+__global__ void __launch_bounds__(256) first_bad_kernel(Bad bad, uint64_t n, unsigned long long* first) {
+  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x)
+    if (bad(i)) { atomicMin(first, (unsigned long long)i); return; }
+}
+// One grid-stride launch of first_bad_kernel over n elements on d.stream, at most 8 blocks per SM; *first must hold all ones.
+template <class Bad>
+int first_bad_launch(spb_ctx* ctx, DeviceState& d, const Bad& bad, uint64_t n, unsigned long long* first) {
+  const unsigned tb = 256;
+  const uint64_t blocks = (n + tb - 1) / tb, cap = (uint64_t)(d.sm_count > 0 ? d.sm_count : 1) * 8;
+  return launch(ctx, d.stream, (unsigned)(blocks < cap ? blocks : cap), tb, 0, first_bad_kernel<Bad>, bad, n, first);
+}
+
 // One device buffer of a host-buffer entry point: slot `slot` of `bytes` bytes. Before the device core runs, its first
 // `in_bytes` are copied from `in`; after it, its first `out_bytes` are copied to `out` (a null pointer: no copy).
 struct Staging {

@@ -423,12 +423,11 @@ int spb_srs_downsize(spb_ctx* ctx, const spb_srs* srs, uint32_t k, spb_srs** out
 
 namespace spb {
 
-// Lowest index i < n whose point fails affine_check, folded into *first (all ones before the launch). Only a thread that finds
-// a bad point touches the atomic, and it stops there: its later indices are larger.
-__global__ void __launch_bounds__(256) srs_check_kernel(const G1Affine* pts, uint64_t n, unsigned long long* first) {
-  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x)
-    if (affine_check(pts[i]) != kPointValid) { atomicMin(first, (unsigned long long)i); return; }
-}
+// a point that fails affine_check (first_bad_kernel's predicate for the params check)
+struct PointBad {
+  const G1Affine* pts;
+  __device__ bool operator()(uint64_t i) const { return affine_check(pts[i]) != kPointValid; }
+};
 
 static const char* point_check_reason(int verdict) {
   switch (verdict) {
@@ -444,11 +443,9 @@ static const char* point_check_reason(int verdict) {
 static int srs_check_points(spb_ctx* ctx, DeviceState& d, const G1Affine* pts, size_t count, size_t* bad, float* ms) {
   unsigned long long* first = (unsigned long long*)slot(ctx, d, "srs_check", sizeof(unsigned long long));
   if (!first) return SPB_ERR_OOM;
-  const unsigned tb = 256;
-  const uint64_t blocks = (count + tb - 1) / tb, cap = (uint64_t)(d.sm_count > 0 ? d.sm_count : 1) * 8;
   SPB_CUDA(ctx, cudaMemsetAsync(first, 0xff, sizeof(unsigned long long), d.stream));
   SPB_CUDA(ctx, cudaEventRecord(d.ev0, d.stream));
-  SPB_TRY(launch(ctx, d.stream, (unsigned)(blocks < cap ? blocks : cap), tb, 0, srs_check_kernel, pts, count, first));
+  SPB_TRY(first_bad_launch(ctx, d, PointBad{pts}, count, first));
   SPB_CUDA(ctx, cudaEventRecord(d.ev1, d.stream));
   unsigned long long h = 0;
   SPB_CUDA(ctx, cudaMemcpyAsync(&h, first, sizeof h, cudaMemcpyDeviceToHost, d.stream));

@@ -105,4 +105,22 @@ SPB_HD int copy_check_row(const CopyArgs& a, uint64_t i, uint32_t* col, uint64_t
   return fp_eq(ntt_ldg(a.values[a.c] + i), ntt_ldg(a.values[*col] + *row)) ? 0 : 1;
 }
 
+// ---- proving-key check (spb_fr_first_noncanonical_dev, spb_sigma_check_dev) ----
+// an element whose stored limbs are not below r: halo2curves' RawBytes read refuses it
+SPB_HD bool fr_noncanonical(const Fr& a) { return !fp_is_canonical(a); }
+
+// The entry s = sigma_c[i] of a key. Returns whether it labels a cell (*col, *row) of the n_cols columns; a fixed point (its own
+// label) needs no decode, and a non-canonical s labels nothing (the arithmetic of a decode assumes reduced inputs). *bad: the
+// entry fails spb_sigma_check_dev's kind 0 (i < usable and it labels no usable cell) or kind 1 (i >= usable and it is not a
+// fixed point).
+SPB_HD bool sigma_check_entry(const SigmaTables& t, uint32_t c, uint64_t i, const Fr& s, uint64_t usable, uint32_t* col, uint64_t* row, bool* bad) {
+  if (fp_eq(s, sigma_label(t, c, i))) { *col = c; *row = i; *bad = false; return true; }
+  const bool ok = fp_is_canonical(s) && sigma_decode(t, s, col, row);
+  *bad = i >= usable || !ok || *row >= usable;
+  return ok;
+}
+// bit of cell (c, i) in a map of n_cols columns, words_per_col 32-bit words each
+SPB_HD uint64_t sigma_map_word(uint64_t words_per_col, uint32_t c, uint64_t i) { return c * words_per_col + (i >> 5); }
+SPB_HD uint32_t sigma_map_bit(uint64_t i) { return 1u << (i & 31u); }
+
 }  // namespace spb

@@ -376,6 +376,33 @@ class Backend:
             out.append((t, [(int(r), int(c2), int(r2)) for _, r, c2, r2 in cells[c * cap:c * cap + min(cap, t)]]))
         return out
 
+    # ---- proving-key check --------------------------------------------------------------------------------
+    def fr_first_noncanonical_dev(self, d_elems, n):
+        """-> the first index i < n whose stored limbs are not below r, or n when every element is canonical"""
+        first = ctypes.c_uint64()
+        self.check(self.lib.spb_fr_first_noncanonical_dev(self.ctx, _p(d_elems), ctypes.c_size_t(n), ctypes.byref(first)), "spb_fr_first_noncanonical_dev")
+        return first.value
+
+    def sigma_check_dev(self, k, d_sigma, usable, cap):
+        """-> per permutation column: three (total, first `cap` rows ascending) for the kinds label, blinding, unlabelled"""
+        m = len(d_sigma)
+        ptrs = (ctypes.c_void_p * max(1, m))(*d_sigma)
+        rows, totals = np.zeros(max(3 * m * cap, 1), dtype=np.uint32), np.zeros(max(3 * m, 1), dtype=np.uint64)
+        self.check(self.lib.spb_sigma_check_dev(self.ctx, ctypes.c_uint32(k), ptrs, ctypes.c_uint32(m), ctypes.c_size_t(usable), ctypes.c_uint32(cap),
+                                                _p(rows), _p(totals)), "spb_sigma_check_dev")
+        out = []
+        for c in range(m):
+            kinds = []
+            for q in range(3):
+                t, j = int(totals[3 * c + q]), 3 * c + q
+                kinds.append((t, [int(r) for r in rows[j * cap:j * cap + min(cap, t)]]))
+            out.append(kinds)
+        return out
+
+    def vec_axpy_dev(self, d_y, alpha, d_x, n):
+        """d_y[i] += alpha * d_x[i]"""
+        self.check(self.lib.spb_vec_axpy_dev(self.ctx, _p(d_y), _p(_fr_array(alpha, 1)), _p(d_x), ctypes.c_size_t(n)), "spb_vec_axpy_dev")
+
     # ---- file <-> device streaming (params / proving-key files) -------------------------------------------
     def read_file_dev(self, path, offset, d_dst, nbytes):
         self.check(self.lib.spb_read_file_dev(self.ctx, path.encode(), ctypes.c_uint64(offset), _p(d_dst), ctypes.c_size_t(nbytes)), "spb_read_file_dev")

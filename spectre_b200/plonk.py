@@ -359,6 +359,11 @@ class DeviceEngine:
     def copy_mismatches(self, values, sigma, usable, cap):
         return self.be.copy_mismatches_dev(self.k, [b.data_ptr() for b in values], [b.data_ptr() for b in sigma], usable, cap)
 
+    # proving-key check
+    def first_noncanonical(self, b, rows): return self.be.fr_first_noncanonical_dev(b.data_ptr(), rows)
+    def sigma_check(self, sigma, usable, cap): return self.be.sigma_check_dev(self.k, [b.data_ptr() for b in sigma], usable, cap)
+    def vec_axpy(self, y, alpha, x, n): self.be.vec_axpy_dev(y.data_ptr(), alpha, x.data_ptr(), n)
+
     # batch ops
     def eval_polynomial(self, b, n, point): return self.be.eval_polynomial_dev(b.data_ptr(), n, point)
     def eval_polynomial_many(self, pairs, n):
@@ -586,11 +591,38 @@ def write_pk(E, pk, path):
     polys(pk.sigma_values, pk.n, m); polys(pk.sigma_polys, pk.n, m); polys(cosets(pk.sigma_cosets, pk.sigma_polys), ext, m)
 
 
-def read_pk(E, cs, path, vk_digest=None, cosets="resident"):
+PK_FORMATS = ("RawBytes", "RawBytesUnchecked")
+
+
+def _point_check(raw):
+    """None for a G1Affine as RawBytes stores it that halo2curves' checked read accepts (canonical coordinates on y^2 = x^3 + 3,
+    or the identity (0, 0)), else the reason it is refused (the texts of the params check, spb_srs_read_file_custom)"""
+    rx, ry = int.from_bytes(raw[:32], "little"), int.from_bytes(raw[32:64], "little")
+    if rx >= P_MOD:
+        return "x is not less than the field modulus"
+    if ry >= P_MOD:
+        return "y is not less than the field modulus"
+    if rx == 0 and ry == 0:
+        return None
+    x, y = _point_from(raw)
+    return None if (y * y - x * x * x - 3) % P_MOD == 0 else "not on the curve"
+
+
+def read_pk(E, cs, path, vk_digest=None, cosets="resident", format="RawBytesUnchecked"):
     """ProvingKey::read: the inverse of write_pk; `cs` plays the role of the concrete circuit's configure().
     cosets="on_demand" reads a lean key from the same file: the coset sections are skipped, never read, and the three l
-    polynomials are rebuilt from their definition. cosets="per_part" reads the same lean key for per-part proofs."""
+    polynomials are rebuilt from their definition. cosets="per_part" reads the same lean key for per-part proofs.
+
+    format="RawBytesUnchecked" (SerdeFormat::RawBytesUnchecked) believes every byte. format="RawBytes" is upstream's checked
+    read: every VK point is checked on the host (coordinates below p, on the curve or the identity) and every polynomial is
+    scanned on the device right after it lands (spb_fr_first_noncanonical_dev: limbs below r). The first failure in file order
+    raises ValueError naming the file, the section and index, the row and the reason; the buffers already read are freed. A
+    lean read never reads the coset sections, so it does not check them either. The read says nothing about whether the key
+    belongs to the params it is used with: that is check_pk."""
     _check_cosets_mode(cosets)
+    if format not in PK_FORMATS:
+        raise ValueError("read_pk: format must be one of %s (the compressed Processed format is not implemented)" % sorted(PK_FORMATS))
+    checked = format == "RawBytes"
     lean = cosets != "resident"
     pk = ProvingKey()
     pk.per_part = cosets == "per_part"
@@ -599,9 +631,16 @@ def read_pk(E, cs, path, vk_digest=None, cosets="resident"):
         k, n_fixed = int.from_bytes(head[:4], "big"), int.from_bytes(head[4:], "big")
         if k != E.k or n_fixed != cs.num_fixed:
             raise ValueError("read_pk: %s is for k = %d with %d fixed columns, expected k = %d with %d" % (path, k, n_fixed, E.k, cs.num_fixed))
-        pts = [_point_from(f.read(64)) for _ in range(n_fixed + len(cs.permutation))]
+        raws = [f.read(64) for _ in range(n_fixed + len(cs.permutation))]
         pos = [f.tell()]
         size = f.seek(0, 2)
+    if checked:
+        for i, raw in enumerate(raws):
+            why = _point_check(raw)
+            if why is not None:
+                what = "fixed commitment %d" % i if i < n_fixed else "sigma commitment %d" % (i - n_fixed)
+                raise ValueError("read_pk: %s: %s: %s" % (path, what, why))
+    pts = [_point_from(raw) for raw in raws]
     n, ext = 1 << k, 1 << E.extended_k
     pk.cs, pk.k, pk.n = cs, k, n
     pk.blinding_factors = cs.blinding_factors(); pk.usable_rows = n - (pk.blinding_factors + 1)
@@ -613,22 +652,33 @@ def read_pk(E, cs, path, vk_digest=None, cosets="resident"):
         pos[0] += 4
         return v
 
-    def poly(rows, skip=False):
+    def poly(rows, what, skip=False):
         if u32() != rows:
             raise ValueError("read_pk: polynomial length mismatch in %s" % path)
         b = None if skip else E.read_from_file(path, pos[0], rows)
         pos[0] += rows * 32
+        if checked and b is not None:
+            bad = E.first_noncanonical(b, rows)
+            if bad < rows:
+                del b
+                raise ValueError("read_pk: %s: %s row %d: not a canonical field element" % (path, what, bad))
         return b
 
-    def polys(count, rows, skip=False):
+    def polys(count, rows, what, skip=False):
         if u32() != count:
             raise ValueError("read_pk: slice length mismatch in %s" % path)
-        bufs = [poly(rows, skip) for _ in range(count)]
+        bufs = [poly(rows, "%s[%d]" % (what, i), skip) for i in range(count)]
         return None if skip else bufs
-    pk.l0, pk.l_last, pk.l_active = poly(ext, lean), poly(ext, lean), poly(ext, lean)
-    pk.fixed_values, pk.fixed_polys, pk.fixed_cosets = polys(n_fixed, n), polys(n_fixed, n), polys(n_fixed, ext, lean)
     m = len(cs.permutation)
-    pk.sigma_values, pk.sigma_polys, pk.sigma_cosets = polys(m, n), polys(m, n), polys(m, ext, lean)
+    try:
+        pk.l0, pk.l_last, pk.l_active = poly(ext, "l0", lean), poly(ext, "l_last", lean), poly(ext, "l_active", lean)
+        pk.fixed_values, pk.fixed_polys = polys(n_fixed, n, "fixed_values"), polys(n_fixed, n, "fixed_polys")
+        pk.fixed_cosets = polys(n_fixed, ext, "fixed_cosets", lean)
+        pk.sigma_values, pk.sigma_polys = polys(m, n, "sigma_values"), polys(m, n, "sigma_polys")
+        pk.sigma_cosets = polys(m, ext, "sigma_cosets", lean)
+    except ValueError:
+        pk.__dict__.clear()                                  # the buffers already read are freed, even while the error is held
+        raise
     if pos[0] != size:
         raise ValueError("read_pk: %d trailing bytes in %s" % (size - pos[0], path))
     pk.l_polys = l_polys(E, n, pk.usable_rows) if lean else None
@@ -994,4 +1044,87 @@ def check_witness(E, pk, instances, advice_columns, theta=None, max_rows=16):
         for c, (total, cells) in enumerate(E.copy_mismatches(cols, pk.sigma_values, usable, max_rows)):
             if total:
                 failures.append(WitnessFailure("copy", c, [r for r, _, _ in cells], total, [(c2, r2) for _, c2, r2 in cells]))
+    return failures
+
+
+# ---- proving-key check --------------------------------------------------------------------------------------------
+class KeyFailure(namedtuple("KeyFailure", "kind index rows total")):
+    """One failing part of a proving key (check_pk). kind and index:
+      "fixed_commitment" / "sigma_commitment" (column): the VK point is not commit_lagrange of the column's values under the
+        engine's params (rows None, total 1);
+      "fixed_poly" / "sigma_poly" (column): the Lagrange rows where the NTT of the stored coefficients differs from the stored
+        values;
+      "fixed_coset" / "sigma_coset" (column), "l_coset" (0 l0, 1 l_last, 2 l_active): resident keys only, the extended rows
+        where the stored coset differs from the coset NTT of the stored coefficients (of l_polys for the l cosets);
+      "sigma_label" / "sigma_blinding" / "sigma_unlabelled" (permutation column): the three kinds of spb_sigma_check_dev, the
+        rows i < u whose sigma labels no usable cell, the rows i >= u that are not fixed points, and the cells no sigma labels.
+    rows: the first failing rows, ascending; total: how many rows fail."""
+
+
+KEY_FAILURE_KINDS = ("fixed_commitment", "sigma_commitment", "fixed_poly", "sigma_poly", "fixed_coset", "sigma_coset", "l_coset", "sigma_label",
+                     "sigma_blinding", "sigma_unlabelled")
+
+
+def check_pk(E, pk, max_rows=16, timings=None):
+    """Audit a proving key against the engine's params and against itself: a list of KeyFailure in the order of
+    KEY_FAILURE_KINDS, ascending by index within a kind; [] for a sound key. Works on every residency mode; nothing is written
+    to the key, and every temporary is freed before it returns.
+
+    Values are the reference: a polynomial is compared as NTT(coefficients) against the values and a coset as the coset NTT of
+    the coefficients against the stored coset, so one corrupted value or coset row is reported as that row. The commitments
+    are recomputed from the values with one batch of nf + m MSMs, so a key made under other params shows as exactly nf + m
+    commitment failures. The row comparisons go through one temporary of at most 2^extended_k rows (n rows for a lean key):
+    recompute, subtract the stored buffer (vec_axpy with -1), report the nonzero rows. pk.vk_digest is not checked.
+    timings: as create_proof's, a dict that gets the wall time of the stages commitments / polys / cosets / sigma."""
+    import time
+    t_last = [time.perf_counter()]
+
+    def lap(name):
+        if timings is not None:
+            E.sync(); t = time.perf_counter(); timings[name] = timings.get(name, 0.0) + t - t_last[0]; t_last[0] = t
+    n, ext = pk.n, 1 << E.extended_k
+    minus_one = fr_mont(R_MOD - 1)
+    nf, m = len(pk.fixed_values), len(pk.sigma_values)
+    failures = []
+    values = pk.fixed_values + pk.sigma_values
+    got = E.commit(halo2.BASIS_G_LAGRANGE, values, n) if values else []
+    for i, (want, have) in enumerate(zip(pk.fixed_commitments + pk.sigma_commitments, got)):
+        if tuple(want) != tuple(have):
+            failures.append(KeyFailure("fixed_commitment" if i < nf else "sigma_commitment", i if i < nf else i - nf, None, 1))
+    lap("commitments")
+
+    def compare(kind, index, tmp, stored, rows):
+        E.vec_axpy(tmp, minus_one, stored, rows)
+        bad, total = E.nonzero_rows(tmp, 0, rows, max_rows)
+        if total:
+            failures.append(KeyFailure(kind, index, bad, total))
+
+    for kind, vals, coeffs in (("fixed_poly", pk.fixed_values, pk.fixed_polys), ("sigma_poly", pk.sigma_values, pk.sigma_polys)):
+        for i, (v, p) in enumerate(zip(vals, coeffs)):
+            tmp = E.clone(p)
+            E.coeff_to_lagrange(tmp)
+            compare(kind, i, tmp, v, n)
+            del tmp
+    lap("polys")
+    if not pk.lean:
+        for kind, coeffs, cosets in (("fixed_coset", pk.fixed_polys, pk.fixed_cosets), ("sigma_coset", pk.sigma_polys, pk.sigma_cosets)):
+            for i, (p, c) in enumerate(zip(coeffs, cosets)):
+                tmp = E.coeff_to_extended(p)
+                compare(kind, i, tmp, c, ext)
+                del tmp
+        ls = l_polys(E, n, pk.usable_rows)
+        for i, c in enumerate((pk.l0, pk.l_last, pk.l_active)):
+            tmp = E.coeff_to_extended(ls[i])
+            compare("l_coset", i, tmp, c, ext)
+            del tmp
+        del ls
+        lap("cosets")
+    if m:
+        report = E.sigma_check(pk.sigma_values, pk.usable_rows, max_rows)
+        for q, kind in enumerate(("sigma_label", "sigma_blinding", "sigma_unlabelled")):
+            for c in range(m):
+                total, rows = report[c][q]
+                if total:
+                    failures.append(KeyFailure(kind, c, rows, total))
+        lap("sigma")
     return failures
