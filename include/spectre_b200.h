@@ -389,9 +389,19 @@ int spb_g1_fixed_base_mul(spb_ctx* ctx, const spb_fr* scalars, size_t n, spb_g1_
  * when the pass declines (malformed program, a target written twice): the caller's program is then run as it is. */
 int spb_test_schedule_program(const uint32_t* program, size_t program_words, uint32_t num_calculations, uint32_t* out_words, size_t out_capacity,
                               size_t* out_count, uint32_t* num_slots, uint32_t* out_calculations);
-/* Elementwise device arithmetic exposed for parity tests of the field/curve layer: op 0 mul, 1 add, 2 sub;
- * field 0 = Fr, 1 = Fq. */
+/* Elementwise device field arithmetic for parity tests of csrc/field.cuh, on raw limbs (field 0 = Fr, 1 = Fq; an Fq element
+ * travels as an spb_fr). Binary: op 0 mul, 1 add, 2 sub. Unary, b unread: 3 sqr, 4 neg, 5 dbl, 6 inv, 7 to_mont, 8 from_mont,
+ * 9 is_canonical (out = 1 or 0 in limb 0). Powers: 10 pow (exponent b as a canonical 256-bit integer), 11 pow_u64 (exponent the
+ * low 64 bits of b). b must be readable for every op. */
 int spb_test_field_op(spb_ctx* ctx, int field, int op, const spb_fr* a, const spb_fr* b, spb_fr* out, size_t n);
+/* out[i] = a[i] * b[i] - c[i] * d[i] through fp_mul_sub_mul (two products under one Montgomery reduction). */
+int spb_test_field_mul_sub_mul(spb_ctx* ctx, int field, const spb_fr* a, const spb_fr* b, const spb_fr* c, const spb_fr* d, spb_fr* out, size_t n);
+/* Elementwise G1 operations of csrc/curve.cuh for parity tests. p, q and out hold n points of four spb_fr each, XYZZ
+ * {x, y, zz, zzz} in Montgomery Fq; an affine operand is the (x, y) of its slot. op 0: p + q (q affine, xyzz_add_mixed);
+ * 1: p + q (xyzz_add); 2: 2p (xyzz_dbl); 3: 2p (p affine, xyzz_dbl_affine); 4: p in affine (out = {x, y, 0, 0}); 5: k[i] * p
+ * (xyzz_mul_u32; k may be NULL for the other ops); 6: affine_check of p's (x, y) (out x limb 0 = the verdict: 0 valid,
+ * 1 x not canonical, 2 y not canonical, 3 off the curve). q must be readable for every op. */
+int spb_test_curve_op(spb_ctx* ctx, int op, const spb_fr* p, const spb_fr* q, const uint32_t* k, spb_fr* out, size_t n);
 /* modular-multiply throughput microbenchmark: `iters` dependent products per thread over `threads` threads, `ilp`
  * independent chains each (1, 2 or 4; ilp | 0x100 = two chains of squarings); returns device milliseconds in *ms. */
 int spb_bench_modmul(spb_ctx* ctx, int field, uint32_t threads, uint32_t iters, int ilp, float* ms);

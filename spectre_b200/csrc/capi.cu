@@ -112,14 +112,49 @@ int stream_device_to_file(spb_ctx* ctx, DeviceState& d, FILE* f, const void* d_s
 
 }  // namespace spb
 
+// The test kernels below inline the field / curve primitives under their own register allocation; the test suite runs them on
+// operand corpora against Python integers and against the same code built for the host (tests/hostemu/hostemu.cpp).
 template <class P>
 __global__ void field_op_kernel(int op, const Fp<P>* a, const Fp<P>* b, Fp<P>* o, size_t n) {
   size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
   if (i >= n) return;
-  Fp<P> x = a[i], y = b[i], r;
-  if (op == 0) r = fp_mul(x, y);
-  else if (op == 1) r = fp_add(x, y);
-  else r = fp_sub(x, y);
+  const Fp<P> x = a[i], y = b[i];
+  Fp<P> r;
+  switch (op) {
+    case 0: r = fp_mul(x, y); break;
+    case 1: r = fp_add(x, y); break;
+    case 2: r = fp_sub(x, y); break;
+    case 3: r = fp_sqr(x); break;
+    case 4: r = fp_neg(x); break;
+    case 5: r = fp_dbl(x); break;
+    case 6: r = fp_inv(x); break;
+    case 7: r = fp_to_mont(x); break;
+    case 8: r = fp_from_mont(x); break;
+    case 9: r = fp_zero<P>(); r.l[0] = fp_is_canonical(x) ? 1u : 0u; break;
+    case 10: r = fp_pow(x, y.l); break;
+    default: r = fp_pow_u64(x, ((uint64_t)y.l[1] << 32) | y.l[0]); break;
+  }
+  o[i] = r;
+}
+template <class P>
+__global__ void field_mul_sub_mul_kernel(const Fp<P>* a, const Fp<P>* b, const Fp<P>* c, const Fp<P>* d, Fp<P>* o, size_t n) {
+  size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+  if (i < n) o[i] = fp_mul_sub_mul(a[i], b[i], c[i], d[i]);
+}
+__device__ __forceinline__ G1Affine xyzz_xy(const G1Xyzz& p) { G1Affine r; r.x = p.x; r.y = p.y; return r; }
+__global__ void curve_op_kernel(int op, const G1Xyzz* p, const G1Xyzz* q, const uint32_t* k, G1Xyzz* o, size_t n) {
+  size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  G1Xyzz r = p[i];
+  switch (op) {
+    case 0: xyzz_add_mixed(r, xyzz_xy(q[i])); break;
+    case 1: xyzz_add(r, q[i]); break;
+    case 2: r = xyzz_dbl(r); break;
+    case 3: r = xyzz_dbl_affine(xyzz_xy(r)); break;
+    case 4: { G1Affine a = xyzz_to_affine(r); r.x = a.x; r.y = a.y; r.zz = fp_zero<FqParams>(); r.zzz = fp_zero<FqParams>(); break; }
+    case 5: r = xyzz_mul_u32(r, k[i]); break;
+    default: { const int v = affine_check(xyzz_xy(r)); r = G1Xyzz{}; r.x.l[0] = (uint32_t)v; break; }
+  }
   o[i] = r;
 }
 
@@ -498,6 +533,7 @@ int spb_divide_by_vanishing_dev(spb_ctx* ctx, const spb_domain* dm, spb_fr* d_a)
 // ---- test utilities ----------------------------------------------------------------------------------------
 int spb_test_field_op(spb_ctx* ctx, int field, int op, const spb_fr* a, const spb_fr* b, spb_fr* out, size_t n) {
   if (!ctx || !a || !b || !out) return SPB_ERR_ARG;
+  if (op < 0 || op > 11) return set_error(ctx, SPB_ERR_ARG, "spb_test_field_op: op %d", op);
   SPB_ENTER(ctx);
   Fr* buf = (Fr*)slot(ctx, d, "test_io", 3 * n * sizeof(Fr));
   if (!buf) return SPB_ERR_OOM;
@@ -506,6 +542,39 @@ int spb_test_field_op(spb_ctx* ctx, int field, int op, const spb_fr* a, const sp
   if (field == 0) SPB_TRY(launch(ctx, d.stream, nblk(n, 128), 128, 0, field_op_kernel<FrParams>, op, (const Fr*)buf, (const Fr*)(buf + n), (Fr*)(buf + 2 * n), n));
   else SPB_TRY(launch(ctx, d.stream, nblk(n, 128), 128, 0, field_op_kernel<FqParams>, op, (const Fq*)buf, (const Fq*)(buf + n), (Fq*)(buf + 2 * n), n));
   SPB_CUDA(ctx, cudaMemcpyAsync(out, buf + 2 * n, n * 32, cudaMemcpyDeviceToHost, d.stream));
+  SPB_CUDA(ctx, cudaStreamSynchronize(d.stream));
+  return 0;
+}
+
+int spb_test_field_mul_sub_mul(spb_ctx* ctx, int field, const spb_fr* a, const spb_fr* b, const spb_fr* c, const spb_fr* dd, spb_fr* out, size_t n) {
+  if (!ctx || !a || !b || !c || !dd || !out) return SPB_ERR_ARG;
+  SPB_ENTER(ctx);
+  Fr* buf = (Fr*)slot(ctx, d, "test_io", 5 * n * sizeof(Fr));
+  if (!buf) return SPB_ERR_OOM;
+  const spb_fr* in[4] = {a, b, c, dd};
+  for (int j = 0; j < 4; j++) SPB_CUDA(ctx, cudaMemcpyAsync(buf + j * n, in[j], n * 32, cudaMemcpyHostToDevice, d.stream));
+  if (field == 0) SPB_TRY(launch(ctx, d.stream, nblk(n, 128), 128, 0, field_mul_sub_mul_kernel<FrParams>, (const Fr*)buf, (const Fr*)(buf + n), (const Fr*)(buf + 2 * n),
+                                 (const Fr*)(buf + 3 * n), (Fr*)(buf + 4 * n), n));
+  else SPB_TRY(launch(ctx, d.stream, nblk(n, 128), 128, 0, field_mul_sub_mul_kernel<FqParams>, (const Fq*)buf, (const Fq*)(buf + n), (const Fq*)(buf + 2 * n),
+                      (const Fq*)(buf + 3 * n), (Fq*)(buf + 4 * n), n));
+  SPB_CUDA(ctx, cudaMemcpyAsync(out, buf + 4 * n, n * 32, cudaMemcpyDeviceToHost, d.stream));
+  SPB_CUDA(ctx, cudaStreamSynchronize(d.stream));
+  return 0;
+}
+
+int spb_test_curve_op(spb_ctx* ctx, int op, const spb_fr* p, const spb_fr* q, const uint32_t* k, spb_fr* out, size_t n) {
+  if (!ctx || !p || !q || !out || (op == 5 && !k)) return SPB_ERR_ARG;
+  if (op < 0 || op > 6) return set_error(ctx, SPB_ERR_ARG, "spb_test_curve_op: op %d", op);
+  SPB_ENTER(ctx);
+  const size_t pb = n * sizeof(G1Xyzz);
+  char* buf = (char*)slot(ctx, d, "test_io", 3 * pb + n * sizeof(uint32_t));
+  if (!buf) return SPB_ERR_OOM;
+  G1Xyzz* dp = (G1Xyzz*)buf; G1Xyzz* dq = dp + n; G1Xyzz* dout = dq + n; uint32_t* dk = (uint32_t*)(dout + n);
+  SPB_CUDA(ctx, cudaMemcpyAsync(dp, p, pb, cudaMemcpyHostToDevice, d.stream));
+  SPB_CUDA(ctx, cudaMemcpyAsync(dq, q, pb, cudaMemcpyHostToDevice, d.stream));
+  if (k) SPB_CUDA(ctx, cudaMemcpyAsync(dk, k, n * sizeof(uint32_t), cudaMemcpyHostToDevice, d.stream));
+  SPB_TRY(launch(ctx, d.stream, nblk(n, 128), 128, 0, curve_op_kernel, op, (const G1Xyzz*)dp, (const G1Xyzz*)dq, (const uint32_t*)(k ? dk : nullptr), dout, n));
+  SPB_CUDA(ctx, cudaMemcpyAsync(out, dout, pb, cudaMemcpyDeviceToHost, d.stream));
   SPB_CUDA(ctx, cudaStreamSynchronize(d.stream));
   return 0;
 }

@@ -417,11 +417,33 @@ class Backend:
         self.check(self.lib.spb_g1_fixed_base_mul(self.ctx, _p(scalars), ctypes.c_size_t(scalars.shape[0]), _p(out)), "spb_g1_fixed_base_mul")
         return out
 
-    def test_field_op(self, field, op, a, b):
-        a = _fr_array(a); b = _fr_array(b, a.shape[0])
+    TEST_FIELD_OPS = {"mul": 0, "add": 1, "sub": 2, "sqr": 3, "neg": 4, "dbl": 5, "inv": 6, "to_mont": 7, "from_mont": 8, "is_canonical": 9,
+                      "pow": 10, "pow_u64": 11}
+    TEST_CURVE_OPS = {"add_mixed": 0, "add": 1, "dbl": 2, "dbl_affine": 3, "to_affine": 4, "mul_u32": 5, "affine_check": 6}
+
+    def test_field_op(self, field, op, a, b=None):
+        """spb_test_field_op; b (exponent for pow / pow_u64) defaults to zeros for the unary ops"""
+        a = _fr_array(a); b = np.zeros_like(a) if b is None else _fr_array(b, a.shape[0])
         out = np.empty_like(a)
-        f = {"fr": 0, "fq": 1}[field]; o = {"mul": 0, "add": 1, "sub": 2}[op]
+        f = {"fr": 0, "fq": 1}[field]; o = self.TEST_FIELD_OPS[op]
         self.check(self.lib.spb_test_field_op(self.ctx, f, o, _p(a), _p(b), _p(out), ctypes.c_size_t(a.shape[0])), "spb_test_field_op")
+        return out
+
+    def test_field_mul_sub_mul(self, field, a, b, c, d):
+        a = _fr_array(a); b, c, d = (_fr_array(x, a.shape[0]) for x in (b, c, d))
+        out = np.empty_like(a)
+        self.check(self.lib.spb_test_field_mul_sub_mul(self.ctx, {"fr": 0, "fq": 1}[field], _p(a), _p(b), _p(c), _p(d), _p(out), ctypes.c_size_t(a.shape[0])),
+                   "spb_test_field_mul_sub_mul")
+        return out
+
+    def test_curve_op(self, op, p, q=None, k=None):
+        """spb_test_curve_op on (n, 16) uint64 XYZZ points; q defaults to zeros, k (uint32 per point) is needed by mul_u32"""
+        p = np.ascontiguousarray(p, dtype=np.uint64).reshape(-1, 16)
+        q = np.zeros_like(p) if q is None else np.ascontiguousarray(q, dtype=np.uint64).reshape(-1, 16)
+        assert q.shape == p.shape
+        k = None if k is None else np.ascontiguousarray(k, dtype=np.uint32).reshape(p.shape[0])
+        out = np.empty_like(p)
+        self.check(self.lib.spb_test_curve_op(self.ctx, self.TEST_CURVE_OPS[op], _p(p), _p(q), _p(k), _p(out), ctypes.c_size_t(p.shape[0])), "spb_test_curve_op")
         return out
 
     def bench_modmul(self, field="fq", threads=132 * 2048, iters=2000, ilp=2):

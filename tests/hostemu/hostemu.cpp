@@ -1,6 +1,7 @@
 // Host build of the DEVICE arithmetic headers, for CPU-only unit tests (tests/test_hostemu.py).
-// Compiled twice: with -DSPB_EMULATE_PTX (the 32-bit-limb PTX carry-chain algorithms, instruction for
-// instruction, with an emulated carry flag) and without (the 64-bit host-glue path).
+// Compiled with -DSPB_EMULATE_PTX (the 32-bit-limb PTX carry-chain algorithms, instruction for instruction, with an
+// emulated carry flag), without it (the 64-bit host-glue path), and with -DSPB_EMULATE_PTX -DSPB_EMULATE_PTX_TRACE
+// (the emulated path recording its carries per call site: tests/arith_corpus.py).
 #include "../../spectre_b200/csrc/curve.cuh"
 #include <string.h>
 using namespace spb;
@@ -34,6 +35,82 @@ void he_mul_u32(G1Affine* out, const G1Affine* p, uint32_t k) { *out = xyzz_to_a
 void he_dbl(G1Affine* out, const G1Affine* p) { *out = xyzz_to_affine(xyzz_dbl(xyzz_from_affine(*p))); }
 int he_on_curve(const G1Affine* p) { return affine_on_curve(*p) ? 1 : 0; }
 void he_jac_roundtrip(G1Affine* out, const G1Affine* p) { G1Jac j = jac_from_affine(*p); G1Xyzz x = xyzz_from_jac(j); *out = jac_to_affine(jac_from_affine(xyzz_to_affine(x))); }
+}
+
+// ---- the host twins of the spb_test_* field / curve hooks (capi.cu), same operation codes -------------------------------
+namespace {
+template <class P> Fp<P> field_op(int op, const Fp<P>& x, const Fp<P>& y) {
+  switch (op) {
+    case 0: return fp_mul(x, y);
+    case 1: return fp_add(x, y);
+    case 2: return fp_sub(x, y);
+    case 3: return fp_sqr(x);
+    case 4: return fp_neg(x);
+    case 5: return fp_dbl(x);
+    case 6: return fp_inv(x);
+    case 7: return fp_to_mont(x);
+    case 8: return fp_from_mont(x);
+    case 9: { Fp<P> r = fp_zero<P>(); r.l[0] = fp_is_canonical(x) ? 1u : 0u; return r; }
+    case 10: return fp_pow(x, y.l);
+    default: return fp_pow_u64(x, ((uint64_t)y.l[1] << 32) | y.l[0]);
+  }
+}
+#if defined(SPB_EMULATE_PTX_TRACE)
+#define SPB_TRACE_MARK() ptx::trace_mark()
+#else
+#define SPB_TRACE_MARK() ((void)0)
+#endif
+template <class P> void field_ops(int op, const Fp256* a, const Fp256* b, Fp256* o, size_t n) {
+  for (size_t i = 0; i < n; i++) {
+    SPB_TRACE_MARK();
+    const Fp<P> x = *(const Fp<P>*)&a[i], y = *(const Fp<P>*)&b[i];
+    *(Fp<P>*)&o[i] = field_op<P>(op, x, y);
+  }
+}
+template <class P> void mul_sub_muls(const Fp256* a, const Fp256* b, const Fp256* c, const Fp256* d, Fp256* o, size_t n) {
+  for (size_t i = 0; i < n; i++) {
+    SPB_TRACE_MARK();
+    *(Fp<P>*)&o[i] = fp_mul_sub_mul(*(const Fp<P>*)&a[i], *(const Fp<P>*)&b[i], *(const Fp<P>*)&c[i], *(const Fp<P>*)&d[i]);
+  }
+}
+G1Affine xy(const G1Xyzz& p) { G1Affine r; r.x = p.x; r.y = p.y; return r; }
+G1Xyzz curve_test_op(int op, const G1Xyzz& p, const G1Xyzz& q, uint32_t k) {
+  G1Xyzz r = p;
+  switch (op) {
+    case 0: xyzz_add_mixed(r, xy(q)); return r;
+    case 1: xyzz_add(r, q); return r;
+    case 2: return xyzz_dbl(p);
+    case 3: return xyzz_dbl_affine(xy(p));
+    case 4: { G1Affine a = xyzz_to_affine(p); r.x = a.x; r.y = a.y; r.zz = fp_zero<FqParams>(); r.zzz = fp_zero<FqParams>(); return r; }
+    case 5: return xyzz_mul_u32(p, k);
+    default: { r = G1Xyzz{}; r.x.l[0] = (uint32_t)affine_check(xy(p)); return r; }
+  }
+}
+}  // namespace
+extern "C" {
+// field 0 = Fr, 1 = Fq; op as spb_test_field_op
+void he_field_op(int field, int op, const Fp256* a, const Fp256* b, Fp256* o, size_t n) {
+  if (field == 0) field_ops<FrParams>(op, a, b, o, n); else field_ops<FqParams>(op, a, b, o, n);
+}
+void he_field_mul_sub_mul(int field, const Fp256* a, const Fp256* b, const Fp256* c, const Fp256* d, Fp256* o, size_t n) {
+  if (field == 0) mul_sub_muls<FrParams>(a, b, c, d, o, n); else mul_sub_muls<FqParams>(a, b, c, d, o, n);
+}
+// op as spb_test_curve_op: points are XYZZ {x, y, zz, zzz}; an affine operand is the (x, y) of its slot
+void he_curve_op(int op, const G1Xyzz* p, const G1Xyzz* q, const uint32_t* k, G1Xyzz* o, size_t n) {
+  for (size_t i = 0; i < n; i++) o[i] = curve_test_op(op, p[i], q[i], k ? k[i] : 0u);
+}
+#if defined(SPB_EMULATE_PTX_TRACE)
+void he_trace_reset() { memset(ptx::g_trace, 0, sizeof ptx::g_trace); }
+// the recorded sites, in table order: file, line, instance, instruction name, seen bits (ptx::kTrace*); returns the number written
+size_t he_trace_read(const char** files, int32_t* lines, int32_t* seqs, const char** ops, uint32_t* seen, size_t cap) {
+  size_t n = 0;
+  for (int i = 0; i < ptx::kTraceCap && n < cap; i++) {
+    const ptx::TraceSite& s = ptx::g_trace[i];
+    if (s.file) { files[n] = s.file; lines[n] = s.line; seqs[n] = s.seq; ops[n] = s.op; seen[n] = s.seen; n++; }
+  }
+  return n;
+}
+#endif
 }
 
 // ---- MSM pipeline, emulated serially with the same per-thread bodies the CUDA kernels call -----------------

@@ -48,8 +48,9 @@ def _edge_and_random(mod, n, rng):
 
 @pytest.mark.parametrize("field", ["fr", "fq"])
 def test_mul_and_sqr_carry_patterns(he, orc, field):
-    """The Karatsuba multiplier / squarer (field.cuh fp_mul_wide, fp_sqr_wide) on operands built to drive every carry:
-    half sums that overflow 2^128, all-ones limbs, equal halves, single-limb values, and 20000 random pairs."""
+    """The interleaved CIOS multiplier (field.cuh fp_mul) and the squarer (fp_sqr: sqr8 then fp_mont_reduce) on operands
+    built to stress their carries: halves near 2^128, all-ones limbs, equal halves, single-limb values, and 20000 random
+    pairs. The per-site carry coverage of these primitives is checked by tests/test_hostemu_carry_coverage.py."""
     mod = pyref.R_MOD if field == "fr" else pyref.P_MOD
     rng = random.Random(99)
     F = (1 << 128) - 1
