@@ -65,7 +65,10 @@ typedef struct spb_domain spb_domain; /* EvaluationDomain<Fr> constants */
 /* One context drives n_dev devices of this process (device_ids == NULL: devices 0..n_dev-1). With n_dev > 1
  * an MSM is sharded by point range over the devices and the partial sums are folded on the host; host-buffer NTTs of
  * 2^16 points and more run six-step across all devices (one NVLink all-to-all), `_dev` NTTs on the first device. Multi-process use (one context per rank, torch.distributed / NCCL between ranks) is
- * what bench.py does. Returns NULL on failure (no CUDA device, bad id). */
+ * what bench.py does. An id may repeat: each entry is a shard with its own stream, workspaces, MSM lanes, twiddle tables and
+ * SRS range, and the entries that name the same device share its memory and SMs (one device, several shards). Such a
+ * context runs every multi-device path on one GPU and computes the same results; it is how the test suite checks those
+ * paths where only one GPU is present. Returns NULL on failure (no CUDA device, bad id). */
 spb_ctx* spb_init(const int* device_ids, int n_dev);
 void spb_shutdown(spb_ctx* ctx);
 /* Free the context's cached device memory -- the grow-only workspaces of MSM, NTT and the provers, and the cached twiddle

@@ -206,14 +206,15 @@ spb_ctx* spb_init(const int* device_ids, int n_dev) {
     if (cudaMallocHost(&d.pinned, d.pinned_cap) != cudaSuccess) { delete ctx; return nullptr; }
     ctx->dev.push_back(d);
   }
-  // several devices: direct NVLink peer copies for the NTT all-to-all and the sharded-MSM scalar scatter
+  // several devices: direct NVLink peer copies for the NTT all-to-all and the sharded-MSM scalar scatter. Two entries that
+  // name the same device (one device, several shards) need no peer access: a device always reaches its own memory.
   ctx->peer_access = ctx->dev.size() > 1;
   for (size_t i = 0; i < ctx->dev.size(); i++)
     for (size_t j = 0; j < ctx->dev.size(); j++) {
-      if (i == j) continue;
+      if (ctx->dev[i].device == ctx->dev[j].device) continue;
       int can = 0;
-      cudaDeviceCanAccessPeer(&can, ctx->dev[i].device, ctx->dev[j].device);
-      if (!can) { ctx->peer_access = false; continue; }
+      if (cudaDeviceCanAccessPeer(&can, ctx->dev[i].device, ctx->dev[j].device) != cudaSuccess) can = 0;
+      if (!can) { ctx->peer_access = false; cudaGetLastError(); continue; }
       cudaSetDevice(ctx->dev[i].device);
       cudaError_t e = cudaDeviceEnablePeerAccess(ctx->dev[j].device, 0);
       if (e != cudaSuccess && e != cudaErrorPeerAccessAlreadyEnabled) ctx->peer_access = false;

@@ -6,6 +6,8 @@ import os
 
 import pytest
 
+from tests.gpu_common import device_lists
+
 pytestmark = pytest.mark.gpu
 
 
@@ -161,18 +163,17 @@ def test_compiled_driver_with_a_lean_key_gives_the_python_bytes(be, orc, tmp_pat
     assert cproof == proof
 
 
-def test_lean_and_resident_keys_agree_on_several_devices_if_available(orc, monkeypatch):
-    """one context over every device: the rebuilt cosets are spread over the devices like every other coset NTT"""
+@pytest.mark.parametrize("ids", device_lists())
+def test_lean_and_resident_keys_agree_on_several_devices(orc, monkeypatch, ids):
+    """one context over several devices: the rebuilt cosets are spread over the devices like every other coset NTT"""
     import torch
-    if torch.cuda.device_count() < 2:
-        pytest.skip("needs two GPUs")
     monkeypatch.setenv("SPB_SHARD_MIN_ROWS", "256")
     monkeypatch.setenv("SPB_SHARD_MIN_LOGN", "8")
     from spectre_b200 import circuits, halo2, plonk
     k, instances = 12, [3, 1, 4]
     cs = circuits.halo2lib_shape(4, 1)
     fixed, adv, copies = circuits.halo2lib_witness(cs, k, instances, lookup_bits=5, groups=200, num_gate_advice=4, num_lookup_advice=1)
-    be2 = halo2.Backend(list(range(min(torch.cuda.device_count(), 8))))
+    be2 = halo2.Backend(ids)
     try:
         E = plonk.DeviceEngine(be2, halo2.ParamsKZG.setup(be2, k, orc.srs_tau()).precompute(), k, cs.degree())
         proofs = [_prove(E, _keygen(E, cs, k, fixed, copies, cosets)[0], instances, adv, seed=5) for cosets in plonk.COSETS_MODES]

@@ -7,7 +7,7 @@ import numpy as np
 import pytest
 
 from tests import pyref
-from tests.gpu_common import be  # noqa: F401
+from tests.gpu_common import be, device_lists  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
@@ -255,13 +255,11 @@ def test_large_msm_tables_known_tau(be, orc):
     assert np.array_equal(affine_of(orc, params.commit_lagrange(a)), orc.commit_lagrange_known_tau(k, a))
 
 
-def test_multi_device_context_if_available(orc):
+@pytest.mark.parametrize("ids", device_lists())
+def test_multi_device_context(orc, ids):
     """n_dev > 1 in one context: SRS sharded by point range, partial sums folded on the host."""
-    import torch
-    if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs")
     from spectre_b200 import halo2
-    be2 = halo2.Backend([0, 1])
+    be2 = halo2.Backend(ids)
     k = 11
     n = 1 << k
     gl = orc.srs_g_lagrange(k, 0, n)

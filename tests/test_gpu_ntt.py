@@ -3,7 +3,7 @@ import numpy as np
 import pytest
 
 from tests import pyref
-from tests.gpu_common import be  # noqa: F401
+from tests.gpu_common import be, device_lists  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
@@ -77,19 +77,13 @@ def test_evaluation_domain_matches_oracle(be, orc, j, k):
             assert orc.fr_ints(ext[i])[0] == sum(c * pow(x, e_, pyref.R_MOD) for e_, c in enumerate(full)) % pyref.R_MOD
 
 
-def test_multi_device_six_step_ntt_if_available(orc):
+@pytest.mark.parametrize("ids", device_lists(power_of_two=True))
+def test_multi_device_six_step_ntt(orc, ids):
     """n_dev > 1 in one context: six-step NTT across devices (column blocks -> first pass -> one all-to-all over
     peer copies -> remaining passes -> strided gather). Must equal the oracle bit for bit, including the fused
     EvaluationDomain variants (zero padding / coset / truncation)."""
-    import torch
-    ndev = torch.cuda.device_count()
-    if ndev < 2:
-        pytest.skip("needs >= 2 GPUs")
     from spectre_b200 import halo2
-    g = 1
-    while g * 2 <= ndev:
-        g *= 2
-    be2 = halo2.Backend(list(range(g)))
+    be2 = halo2.Backend(ids)
     for k in (16, 17, 20, 22, 23):
         a = orc.fr_random_chacha(1 << k, 0x5eed0200 + k)
         w = _omega(orc, k)

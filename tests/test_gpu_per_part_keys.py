@@ -8,6 +8,8 @@ import os
 import numpy as np
 import pytest
 
+from tests.gpu_common import device_lists
+
 pytestmark = pytest.mark.gpu
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -248,19 +250,18 @@ def test_compiled_driver_with_a_per_part_key_gives_the_python_bytes(be, orc, tmp
     assert cproof == proof
 
 
-def test_per_part_and_resident_keys_agree_on_several_devices_if_available(orc, monkeypatch):
-    """one context over every device: the part transforms are spread over the devices and the part passes and scatter are
+@pytest.mark.parametrize("ids", device_lists())
+def test_per_part_and_resident_keys_agree_on_several_devices(orc, monkeypatch, ids):
+    """one context over several devices: the part transforms are spread over the devices and the part passes and scatter are
     sharded by rows"""
     import torch
-    if torch.cuda.device_count() < 2:
-        pytest.skip("needs two GPUs")
     monkeypatch.setenv("SPB_SHARD_MIN_ROWS", "256")
     monkeypatch.setenv("SPB_SHARD_MIN_LOGN", "8")
     from spectre_b200 import circuits, halo2, plonk
     k, instances = 12, [3, 1, 4]
     cs = circuits.halo2lib_shape(4, 1)
     fixed, adv, copies = circuits.halo2lib_witness(cs, k, instances, lookup_bits=5, groups=200, num_gate_advice=4, num_lookup_advice=1)
-    be2 = halo2.Backend(list(range(min(torch.cuda.device_count(), 8))))
+    be2 = halo2.Backend(ids)
     try:
         E = plonk.DeviceEngine(be2, halo2.ParamsKZG.setup(be2, k, orc.srs_tau()).precompute(), k, cs.degree())
         proofs = [_prove(E, plonk.keygen(E, cs, k, fixed, copies, cosets=mode), instances, adv, seed=5) for mode in ("resident", "per_part")]

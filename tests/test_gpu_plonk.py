@@ -5,7 +5,7 @@ import numpy as np
 import pytest
 
 from tests import pyref
-from tests.gpu_common import be  # noqa: F401
+from tests.gpu_common import be, device_lists  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
@@ -254,14 +254,12 @@ def test_k23_proof_equals_the_contract_accepted_fixture(be, orc, kats, path):
     torch.cuda.empty_cache()
 
 
-def test_proof_with_msm_sharded_over_two_devices_if_available(orc, monkeypatch):
+@pytest.mark.parametrize("ids", device_lists())
+def test_proof_with_msm_sharded_over_several_devices(orc, monkeypatch, ids):
     """One context driving several GPUs: every commitment of create_proof is an MSM sharded by point range (scalar ranges
     peer-copied over NVLink), the quotient kernels run on row ranges and the NTTs on whole polynomials spread over the
     devices (all through peer access to the first device's buffers; thresholds lowered so that this small circuit is
     actually sharded); the proof bytes do not change."""
-    import torch
-    if torch.cuda.device_count() < 2:
-        pytest.skip("needs two GPUs")
     monkeypatch.setenv("SPB_SHARD_MIN_ROWS", "256")
     monkeypatch.setenv("SPB_SHARD_MIN_LOGN", "8")
     from spectre_b200 import circuits, halo2, plonk
@@ -270,7 +268,7 @@ def test_proof_with_msm_sharded_over_two_devices_if_available(orc, monkeypatch):
     k, instances = 12, [3, 1, 4]
     cs = circuits.halo2lib_shape(4, 1)
     fixed, adv, copies = circuits.halo2lib_witness(cs, k, instances, lookup_bits=5, groups=200, num_gate_advice=4, num_lookup_advice=1)
-    be2 = halo2.Backend(list(range(min(torch.cuda.device_count(), 8))))
+    be2 = halo2.Backend(ids)
     try:
         proofs = []
         for E in (plonk.DeviceEngine(be2, halo2.ParamsKZG.setup(be2, k, orc.srs_tau()).precompute(), k, cs.degree()), OracleEngine(k, cs.degree())):
@@ -281,18 +279,17 @@ def test_proof_with_msm_sharded_over_two_devices_if_available(orc, monkeypatch):
         be2.close()
 
 
+@pytest.mark.parametrize("ids", device_lists())
 @pytest.mark.parametrize("k", [10, 13])
-def test_grand_products_sharded_by_row_range_over_the_devices_if_available(orc, monkeypatch, k):
+def test_grand_products_sharded_by_row_range_over_the_devices(orc, monkeypatch, k, ids):
     """SURVEY.md 8e "grand product": on a context over several devices the permutation and lookup product columns are built per
     row range (terms, batch inversion and local products in each device's HBM, inputs read over NVLink), the range totals are the
     one exchange, and the seeded scans write their slices of z into the first device's buffer: the columns -- blinding tail and
     the chained last_z included -- equal the oracle's, i.e. the one-device scan, bit for bit."""
     import torch
-    if torch.cuda.device_count() < 2:
-        pytest.skip("needs two GPUs")
     monkeypatch.setenv("SPB_SHARD_MIN_ROWS", "256")
     from spectre_b200 import halo2
-    be2 = halo2.Backend(list(range(min(torch.cuda.device_count(), 8))))
+    be2 = halo2.Backend(ids)
     try:
         n, n_cols, chunk, n_blinds = 1 << k, 5, 2, 5
         values = [orc.fr_random_chacha(n, 100 + c) for c in range(n_cols)]

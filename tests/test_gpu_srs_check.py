@@ -13,7 +13,7 @@ import subprocess
 import numpy as np
 import pytest
 
-from tests.gpu_common import be  # noqa: F401
+from tests.gpu_common import be, device_lists  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
@@ -215,14 +215,12 @@ def test_context_reads_a_valid_file_after_a_rejection(be, orc, k9):
     assert np.array_equal(orc.g1_to_affine(params.commit(poly)), orc.commit_known_tau(poly))
 
 
-def test_two_devices_report_the_global_index(orc, k9):
-    """each shard is checked on its own device; a bad point in the second shard (points 256..511 of 512) is named by its
-    index in the file"""
-    import torch
-    if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs")
+@pytest.mark.parametrize("ids", device_lists())
+def test_several_devices_report_the_global_index(orc, k9, ids):
+    """each shard is checked on its own device; a bad point in a shard after the first (on two devices, points 256..511 of
+    512) is named by its index in the file"""
     from spectre_b200 import halo2
-    be2 = halo2.Backend([0, 1])
+    be2 = halo2.Backend(ids)
     try:
         for basis, i in (("g", 300), ("g_lagrange", 511), ("g", 255)):
             off = k9.g1_offset(basis, i)
