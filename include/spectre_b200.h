@@ -379,8 +379,10 @@ typedef struct spb_shplonk spb_shplonk;
 int spb_shplonk_begin_dev(spb_ctx* ctx, const spb_srs* srs, size_t n, const spb_rotation_set* sets, uint32_t n_sets, const spb_fr* y, const spb_fr* v,
                           spb_g1* h_commitment, spb_shplonk** out);
 /* After squeezing u: L(X) = sum_i v^(s-1-i) Z_{T\S_i}(u) sum_j y^(m_i-1-j) (P_ij(X) - R_ij(u)) - Z_T(u) h(X); commits
- * L(X) / (X - u) / Z_{T\S_0}(u). Consumes the handle (also on error). */
+ * L(X) / (X - u) / Z_{T\S_0}(u). Consumes the handle (also on error, a null argument included). */
 int spb_shplonk_finish_dev(spb_ctx* ctx, spb_shplonk* s, const spb_fr* u, spb_g1* commitment);
+/* Releases an open handle without finishing it (a caller that fails between the two calls). While a handle is open the
+ * context's SHPLONK workspace is held: a second handle allocates its own buffers, and spb_release_workspace fails. */
 void spb_shplonk_abort(spb_ctx* ctx, spb_shplonk* s);
 
 /* ---- test / bench utilities -------------------------------------------------------------------------------- */

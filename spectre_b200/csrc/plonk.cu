@@ -344,8 +344,9 @@ int spb_shplonk_begin_dev(spb_ctx* ctx, const spb_srs* srs, size_t n, const spb_
 }
 
 int spb_shplonk_finish_dev(spb_ctx* ctx, spb_shplonk* s, const spb_fr* u, spb_g1* commitment) {
-  if (!ctx) return SPB_ERR_ARG;
-  if (!s || !u || !commitment) return set_error(ctx, SPB_ERR_ARG, "spb_shplonk_finish_dev: null argument");
+  // the handle is consumed on every return, this one included: otherwise it would keep the context's slots busy for good
+  if (!ctx) { if (s) spb_shplonk_abort(s->ctx, s); return SPB_ERR_ARG; }
+  if (!s || !u || !commitment) { spb_shplonk_abort(ctx, s); return set_error(ctx, SPB_ERR_ARG, "spb_shplonk_finish_dev: null argument"); }
   const Fr uu = fr_load(u);
   const size_t n = s->n;
   const uint32_t n_sets = (uint32_t)s->sets.size();

@@ -338,9 +338,15 @@ class Backend:
         return out, h
 
     def shplonk_finish_dev(self, handle, u):
+        """Consumes the handle, also when it raises."""
         out = np.empty(12, dtype=np.uint64)
         self.check(self.lib.spb_shplonk_finish_dev(self.ctx, handle, _p(_fr_array(u, 1)), _p(out)), "spb_shplonk_finish_dev")
         return out
+
+    def shplonk_abort_dev(self, handle):
+        """spb_shplonk_abort: release a handle of shplonk_begin_dev that will not be finished (its workspace goes back to the context)"""
+        self.lib.spb_shplonk_abort.restype = None
+        self.lib.spb_shplonk_abort(self.ctx, handle)
 
     def permute_expression_pair_dev(self, d_input, d_table, usable, d_permuted_input, d_permuted_table):
         """lookup::prover::permute_expression_pair on device buffers; raises like Error::ConstraintSystemFailure."""

@@ -378,6 +378,7 @@ class DeviceEngine:
         return halo2.jacobian_to_affine_ints(c), h
     def shplonk_finish(self, state, u):
         return halo2.jacobian_to_affine_ints(self.be.shplonk_finish_dev(state, u))
+    def shplonk_abort(self, state): self.be.shplonk_abort_dev(state)
 
 
 def lagrange_to_coeff_many(E, bufs):
@@ -981,9 +982,13 @@ def create_proof(E, pk, instances, advice_columns, rng, transcript, timings=None
     y2 = fr_mont(transcript.squeeze_challenge())
     v = fr_mont(transcript.squeeze_challenge())
     h1, state = E.shplonk_begin(sets, y2, v)
-    transcript.write_ec_point(h1)
-    u = fr_mont(transcript.squeeze_challenge())
-    transcript.write_ec_point(E.shplonk_finish(state, u))
+    try:
+        transcript.write_ec_point(h1)
+        u = fr_mont(transcript.squeeze_challenge())
+    except BaseException:                                     # KeyboardInterrupt too: an open handle holds the context's workspace
+        E.shplonk_abort(state)
+        raise
+    transcript.write_ec_point(E.shplonk_finish(state, u))    # finish consumes the handle, also when it raises
     lap("shplonk")
     return bytes(transcript.proof)
 

@@ -67,6 +67,7 @@ struct spb_shplonk {
 };
 
 static const int kThreads = 4;
+static int g_open_shplonk = 0;                        // spb_shplonk handles begun and not yet finished or aborted
 static int fail(spb_ctx* ctx, int code, const char* msg) { if (ctx) ctx->last_error = msg; return code; }
 static void to_jac(const g1a& a, spb_g1* out) {
   g1a gen; orc_g1_generator(&gen);                       // generator x = 1 in Montgomery form = the Fq "one"
@@ -188,17 +189,26 @@ int spb_shplonk_begin_dev(spb_ctx* ctx, const spb_srs* srs, size_t n, const spb_
   orc_shplonk_quotient(n, os.data(), n_sets, &s->y, &s->v, s->h_x.data());
   int rc = spb_msm_dev(ctx, srs, SPB_BASIS_G, (const spb_fr*)s->h_x.data(), n, h_commitment);
   if (rc) { delete s; return rc; }
+  g_open_shplonk++;
   *out = s;
   return 0;
 }
 int spb_shplonk_finish_dev(spb_ctx* ctx, spb_shplonk* s, const spb_fr* u, spb_g1* commitment) {
+  // the header's contract: the handle is consumed on every return, a null argument included
+  if (!s || !u || !commitment) { spb_shplonk_abort(ctx, s); return fail(ctx, SPB_ERR_ARG, "spb_shplonk_finish_dev: null argument"); }
   std::vector<fe> fin(s->n - 1);
   auto os = s->sets();
   int rc = orc_shplonk_linearisation(s->n, os.data(), (uint32_t)os.size(), &s->y, &s->v, (const fe*)u, s->h_x.data(), fin.data());
   if (rc == 0) rc = spb_msm_dev(ctx, s->srs, SPB_BASIS_G, (const spb_fr*)fin.data(), s->n - 1, commitment);
   else rc = fail(ctx, SPB_ERR_ARG, "abi shim: evaluations inconsistent with the polynomials");
-  delete s;
+  spb_shplonk_abort(ctx, s);
   return rc;
 }
-void spb_shplonk_abort(spb_ctx*, spb_shplonk* s) { delete s; }
+void spb_shplonk_abort(spb_ctx*, spb_shplonk* s) {
+  if (!s) return;
+  g_open_shplonk--;
+  delete s;
+}
+// test hook of the shim alone: the number of spb_shplonk handles begun and not yet consumed
+int spb_shim_open_shplonk_handles(void) { return g_open_shplonk; }
 }

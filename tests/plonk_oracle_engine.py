@@ -86,6 +86,7 @@ class OracleEngine:
     def shplonk_finish(self, state, u):
         hs, y, v, h_x = state
         return _aff(orc.commit_known_tau(orc.shplonk_linearisation(self.n, hs, y, v, u, h_x)))
+    def shplonk_abort(self, state): pass                       # the state is host memory: nothing to release
 
 
 class SeededRng:
@@ -100,3 +101,21 @@ class SeededRng:
             return np.zeros((0, 4), dtype=np.uint64)
         self.counter += 1
         return orc.fr_random_chacha(count, (self.seed << 32) + self.counter)
+
+
+class FailingTranscript:
+    """An EvmTranscriptWrite that raises `exc` on its `fail_at`-th write_ec_point call (counting from 0); `fail_at=None` never
+    raises and only counts. create_proof writes the SHPLONK h commitment as its second-to-last point and the opening as its last."""
+
+    def __init__(self, vk_digest, fail_at=None, exc=RuntimeError):
+        from spectre_b200.transcript import EvmTranscriptWrite
+        self.inner, self.fail_at, self.exc, self.points = EvmTranscriptWrite(vk_digest), fail_at, exc, 0
+
+    def write_ec_point(self, xy):
+        if self.points == self.fail_at:
+            raise self.exc("transcript failure injected at point %d" % self.points)
+        self.points += 1
+        return self.inner.write_ec_point(xy)
+
+    def __getattr__(self, name):
+        return getattr(self.inner, name)

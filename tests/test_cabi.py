@@ -163,3 +163,49 @@ def test_every_entry_point_survives_null_arguments(libpath):
     p = subprocess.run([sys.executable, "-c", prog] + todo, capture_output=True, text=True, timeout=120)
     done = [l.split()[1] for l in p.stdout.splitlines() if l.startswith("ok ")]
     assert p.returncode == 0 and done == todo, "crashed in %s" % (todo[len(done)] if len(done) < len(todo) else p.stderr[-300:])
+
+
+def test_shplonk_finish_consumes_the_handle_on_a_null_argument(orc, tmp_path):
+    """include/spectre_b200.h: spb_shplonk_finish_dev "consumes the handle (also on error)", a null `u` or `commitment`
+    included, so a caller that hands its handle to finish never aborts it as well (the C++ driver's OpenGuard lets go of it
+    before the call). Checked on the CPU stand-in of the ABI (tests/abi_shim), which counts the open handles."""
+    import numpy as np
+    ref_dir = os.path.join(ROOT, "oracle", "_ref")
+    shim = os.path.join(str(tmp_path), "libspb_shim.so")
+    subprocess.check_call(["g++", "-std=c++17", "-O1", "-fPIC", "-shared", "-o", shim, os.path.join(ROOT, "tests", "abi_shim", "shim.cpp"),
+                           "-L" + ref_dir, "-lhalo2_oracle", "-Wl,-rpath," + ref_dir])
+    lib = ctypes.CDLL(shim)
+    lib.spb_init.restype = ctypes.c_void_p
+    ctx = ctypes.c_void_p(lib.spb_init(None, 0))
+    srs = ctypes.c_void_p()
+    tau = orc.srs_tau()
+    assert lib.spb_srs_setup(ctx, 4, tau.ctypes.data_as(ctypes.c_void_p), ctypes.byref(srs)) == 0
+
+    class _Set(ctypes.Structure):
+        _fields_ = [("points", ctypes.c_void_p), ("n_points", ctypes.c_uint32), ("d_polys", ctypes.c_void_p), ("n_polys", ctypes.c_uint32), ("evals", ctypes.c_void_p)]
+    n = 16
+    poly = orc.fr_random_chacha(n, 7)
+    pt, y, v, u = orc.fr_random_chacha(4, 8)
+    ev = orc.eval_polynomial(poly, pt)
+    ptrs = (ctypes.c_void_p * 1)(poly.ctypes.data)
+    rs = _Set(pt.ctypes.data, 1, ctypes.cast(ptrs, ctypes.c_void_p).value, 1, ev.ctypes.data)
+    out = np.empty(12, dtype=np.uint64)
+    vp = lambda a: a.ctypes.data_as(ctypes.c_void_p)
+
+    def begin():
+        h = ctypes.c_void_p()
+        assert lib.spb_shplonk_begin_dev(ctx, srs, ctypes.c_size_t(n), ctypes.byref(rs), 1, vp(y), vp(v), vp(out), ctypes.byref(h)) == 0
+        return h
+    for bad_u, bad_out in ((None, vp(out)), (vp(u), None)):
+        h = begin()
+        assert lib.spb_shim_open_shplonk_handles() == 1
+        assert lib.spb_shplonk_finish_dev(ctx, h, bad_u, bad_out) != 0
+        assert lib.spb_shim_open_shplonk_handles() == 0
+    h = begin()
+    assert lib.spb_shplonk_finish_dev(ctx, h, vp(u), vp(out)) == 0
+    assert lib.spb_shim_open_shplonk_handles() == 0
+    h = begin()
+    lib.spb_shplonk_abort(ctx, h)
+    assert lib.spb_shim_open_shplonk_handles() == 0
+    lib.spb_srs_free(ctx, srs)
+    lib.spb_shutdown(ctx)

@@ -288,6 +288,44 @@ def test_create_proof_argument_errors(orc):
         plonk.create_proof(E, pk, [[1]], [adv, adv], SeededRng(1), new_t())
 
 
+@pytest.mark.parametrize("exc", [RuntimeError, KeyboardInterrupt])
+def test_create_proof_aborts_the_open_shplonk_handle_when_the_transcript_raises(orc, exc):
+    """Between shplonk_begin and shplonk_finish create_proof writes h and squeezes u; an exception there (an interrupt too)
+    aborts the open handle exactly once, and one raised by the final write (after finish consumed the handle) aborts nothing."""
+    from tests.plonk_oracle_engine import FailingTranscript
+    k = 6
+    cs = plonk_circuits.aggregation_shape()
+    fixed, adv, copies = plonk_circuits.aggregation_witness(cs, k, [1], lookup_bits=3, groups=4)
+
+    class Recording(OracleEngine):
+        def __init__(self, *a):
+            super().__init__(*a)
+            self.log = []
+        def shplonk_begin(self, *a):
+            out = super().shplonk_begin(*a)
+            self.log.append("begin")
+            return out
+        def shplonk_finish(self, *a):
+            self.log.append("finish")
+            return super().shplonk_finish(*a)
+        def shplonk_abort(self, state):
+            self.log.append("abort")
+
+    E = Recording(k, cs.degree())
+    pk = plonk.keygen(E, cs, k, fixed, copies)
+    count = FailingTranscript(pk.vk_digest)
+    plonk.create_proof(E, pk, [[1]], [adv], SeededRng(1), count)
+    assert E.log == ["begin", "finish"]
+    E.log.clear()
+    with pytest.raises(exc):
+        plonk.create_proof(E, pk, [[1]], [adv], SeededRng(1), FailingTranscript(pk.vk_digest, count.points - 2, exc))
+    assert E.log == ["begin", "abort"]
+    E.log.clear()
+    with pytest.raises(exc):
+        plonk.create_proof(E, pk, [[1]], [adv], SeededRng(1), FailingTranscript(pk.vk_digest, count.points - 1, exc))
+    assert E.log == ["begin", "finish"]
+
+
 def test_proving_key_file_round_trip(orc, tmp_path):
     """ProvingKey::write / ::read in upstream's RawBytesUnchecked layout (spectre_b200/plonk.py write_pk / read_pk): the key
     read back proves to the same bytes as the key it was written from, and a file for another shape is refused."""
