@@ -385,6 +385,33 @@ int spb_shplonk_finish_dev(spb_ctx* ctx, spb_shplonk* s, const spb_fr* u, spb_g1
  * context's SHPLONK workspace is held: a second handle allocates its own buffers, and spb_release_workspace fails. */
 void spb_shplonk_abort(spb_ctx* ctx, spb_shplonk* s);
 
+/* ---- BN254 pairing ([UPSTREAM] halo2curves src/bn256/engine.rs: multi_miller_loop, final_exponentiation; reached by
+ * halo2's KZG verifier, poly/kzg/strategy.rs) ------------------------------------------------------------------------------ */
+/* A G2 affine point as the params file's G2 trailer stores it: x.c0, x.c1, y.c0, y.c1 (Fq2 = Fq[u]/(u^2 + 1)), Montgomery
+ * limbs; the identity is (0, 0). A Gt value: the 12 Fq coefficients of Fq12 in halo2curves' order c0.c0.c0, c0.c0.c1, ...,
+ * c1.c2.c1 (tower Fq6 = Fq2[v]/(v^3 - (9 + u)), Fq12 = Fq6[w]/(w^2 - v)), Montgomery limbs. */
+typedef struct { spb_fq x[2], y[2]; } spb_g2_affine;
+typedef struct { spb_fq c[12]; } spb_gt;
+/* *out = prod_i e(p[i], q[i]) for the optimal ate pairing e: the product of the Miller values raised to (p^12 - 1) / r, so a
+ * pairing equals upstream's `Bn256::pairing`. A pair in which either point is the identity contributes one; n = 0 gives one.
+ * Every input is checked on the device first: G1 points as the checked params read checks them (coordinates below p, on
+ * y^2 = x^3 + 3, or the identity), G2 points likewise on the twist y^2 = x^3 + 3/(9+u) and in the order-r subgroup ([r]Q = O).
+ * The first invalid input in the order p[0], q[0], p[1], q[1], ... gives SPB_ERR_DATA with its name, index and reason in the
+ * error text, e.g. "q[17]: not in the r-torsion subgroup" or "p[3]: not on the curve", and *out is untouched.
+ * One launch sequence on the context's first device (also when it lists several): the check, one Miller-loop thread per pair,
+ * one final-exponentiation thread; 3 kernel launches (spb_kernel_launches) whatever n. Synchronous: the stream contract of
+ * the host-buffer entry points; spb_last_device_ms gives the device time of the three kernels. NULL context or out, or NULL
+ * p / q with n > 0: SPB_ERR_ARG. The first call makes the CUDA context reserve the kernels' per-thread stacks for every thread
+ * the GPU can hold (826 MiB on an H100 80GB HBM3), which the context keeps until it is destroyed. */
+int spb_pairing(spb_ctx* ctx, const spb_g1_affine* p, const spb_g2_affine* q, size_t n, spb_gt* out);
+/* n_checks independent pairing checks in one launch sequence: ok[j] = 1 iff prod_{i<m} e(p[j*m+i], q[j*m+i]) == 1, else 0.
+ * A KZG opening is one check of m = 2 pairs, e(P1, [1]_2) e(P2, -[s]_2) = 1; a batch of proofs gets one verdict per proof.
+ * Inputs are checked as in spb_pairing over all m * n_checks pairs (SPB_ERR_DATA naming the first invalid one, ok untouched);
+ * then one Miller-loop thread per pair and one final-exponentiation thread per check: 3 kernel launches whatever m and
+ * n_checks. m = 0 gives ok[j] = 1 for every check without touching the device; n_checks = 0 does nothing. NULL context, NULL
+ * ok with n_checks > 0, or NULL p / q with m n_checks > 0: SPB_ERR_ARG. spb_last_device_ms as for spb_pairing. */
+int spb_pairing_check_batch(spb_ctx* ctx, const spb_g1_affine* p, const spb_g2_affine* q, size_t m, size_t n_checks, int32_t* ok);
+
 /* ---- test / bench utilities -------------------------------------------------------------------------------- */
 /* out[i] = scalars[i] * G1 (affine), computed on the device */
 int spb_g1_fixed_base_mul(spb_ctx* ctx, const spb_fr* scalars, size_t n, spb_g1_affine* out);

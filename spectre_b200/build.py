@@ -17,7 +17,7 @@ VARIANT = os.environ.get("SPB_BUILD_VARIANT", "")
 EXTRA_FLAGS = os.environ.get("SPB_BUILD_FLAGS", "").split() if VARIANT else []
 OUT = os.path.join(HERE, "libspectre_b200%s.so" % ("_" + VARIANT if VARIANT else ""))
 OBJDIR = os.path.join(HERE, "_obj" + ("_" + VARIANT if VARIANT else ""))
-SOURCES = ["capi.cu", "ntt.cu", "msm.cu", "poly.cu", "quotient.cu", "lookup.cu", "plonk.cu", "witness.cu"]
+SOURCES = ["capi.cu", "ntt.cu", "msm.cu", "poly.cu", "quotient.cu", "lookup.cu", "plonk.cu", "witness.cu", "pairing.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
          "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr", "-cudart", "static"]

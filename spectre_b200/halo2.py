@@ -10,6 +10,8 @@ the reference's own use of them (reference call sites: lightclient-circuits/src/
     halo2_proofs::poly::EvaluationDomain          -> EvaluationDomain(j, k)
     halo2_proofs::poly::kzg::commitment::ParamsKZG-> ParamsKZG.setup / .from_parts / .read_custom / .commit / .commit_lagrange
     arithmetic::{eval_polynomial, kate_division}, ff::BatchInvert -> same names
+    halo2curves::bn256 multi_miller_loop + final_exponentiation -> Backend.pairing / Backend.pairing_check_batch
+    halo2_proofs::poly::kzg::commitment::ParamsVerifierKZG -> ParamsVerifierKZG, ParamsKZG.verifier_params
 
 Field elements are numpy uint64 arrays (..., 4) holding halo2curves' in-memory Montgomery limbs; G1Affine is
 (..., 8) = x‖y with identity (0,0); G1 (Jacobian) is (12,) = x‖y‖z.
@@ -80,6 +82,14 @@ def _fr_array(a, n=None):
     if n is not None:
         assert a.shape[0] == n, "length mismatch"
     return a
+
+
+def _pair_arrays(ps, qs):
+    ps = np.ascontiguousarray(ps, dtype=np.uint64).reshape(-1, 8)
+    qs = np.ascontiguousarray(qs, dtype=np.uint64).reshape(-1, 16)
+    if ps.shape[0] != qs.shape[0]:
+        raise ValueError("pairing: %d G1 points but %d G2 points" % (ps.shape[0], qs.shape[0]))
+    return ps, qs
 
 
 class Backend:
@@ -168,6 +178,26 @@ class Backend:
         out = np.empty(12, dtype=np.uint64)
         self.check(self.lib.spb_msm_raw(self.ctx, _p(coeffs), _p(bases), ctypes.c_size_t(coeffs.shape[0]), _p(out)), "spb_msm_raw")
         return out
+
+    # ---- pairing (halo2curves bn256 engine) ------------------------------------------------------------
+    def pairing(self, ps, qs):
+        """prod_i e(ps[i], qs[i]) (spb_pairing): ps (n, 8) G1 affine as best_multiexp takes them, qs (n, 16) G2 affine as
+        ParamsKZG.get_g2 returns them. Returns the 12 Fq values of Gt, (12, 4) Montgomery limbs in the order c0.c0.c0 ... c1.c2.c1.
+        An invalid input raises BackendError naming it (SPB_ERR_DATA)."""
+        ps, qs = _pair_arrays(ps, qs)
+        out = np.empty((12, 4), dtype=np.uint64)
+        self.check(self.lib.spb_pairing(self.ctx, _p(ps), _p(qs), ctypes.c_size_t(ps.shape[0]), _p(out)), "spb_pairing")
+        return out
+
+    def pairing_check_batch(self, ps, qs, m):
+        """spb_pairing_check_batch: check j holds iff prod_{i<m} e(ps[j m + i], qs[j m + i]) == 1; a list of len(ps) / m bools"""
+        ps, qs = _pair_arrays(ps, qs)
+        if m <= 0 or ps.shape[0] % m:
+            raise ValueError("pairing_check_batch: %d pairs do not split into checks of m = %d" % (ps.shape[0], m))
+        n_checks = ps.shape[0] // m
+        ok = np.zeros(max(n_checks, 1), dtype=np.int32)
+        self.check(self.lib.spb_pairing_check_batch(self.ctx, _p(ps), _p(qs), ctypes.c_size_t(m), ctypes.c_size_t(n_checks), _p(ok)), "spb_pairing_check_batch")
+        return [bool(v) for v in ok[:n_checks]]
 
     # ---- batch ops -------------------------------------------------------------------------------------
     def batch_invert(self, a):
@@ -638,6 +668,14 @@ class ParamsKZG:
         self.be.check(self.be.lib.spb_srs_get_g2(self.be.ctx, self.h, _p(g2), _p(s_g2)), "spb_srs_get_g2")
         return g2, s_g2
 
+    def verifier_params(self):
+        """ParamsKZG::verifier_params: what a KZG verifier needs, g[0] and the G2 trailer. A handle without G2 points (one made by
+        setup, which does not compute them) raises ValueError: give them with set_g2 first."""
+        g2, s_g2 = self.get_g2()
+        if not g2.any() or not s_g2.any():
+            raise ValueError("verifier_params: the params hold no G2 points; set_g2 first")
+        return ParamsVerifierKZG(self.get_g(0, 1)[0], g2, s_g2)
+
     def __del__(self):
         try:
             if self.be.ctx:
@@ -690,6 +728,17 @@ class ParamsKZG:
         out = np.empty((count, 8), dtype=np.uint64)
         self.be.check(self.be.lib.spb_srs_download(self.be.ctx, self.h, basis, ctypes.c_size_t(start), ctypes.c_size_t(count), _p(out)), "spb_srs_download")
         return out
+
+
+class ParamsVerifierKZG:
+    """ParamsVerifierKZG<Bn256> (upstream's name for the verifier's part of the params): g = g[0] (uint64[8], G1 affine),
+    g2 = [1]_2 and s_g2 = [s]_2 (uint64[16] each, the params file's G2 trailer layout), all Montgomery limbs. Made by
+    ParamsKZG.verifier_params, or directly from constants (a verifier contract's G2 words, say)."""
+
+    def __init__(self, g, g2, s_g2):
+        self.g = np.ascontiguousarray(g, dtype=np.uint64).reshape(8).copy()
+        self.g2 = np.ascontiguousarray(g2, dtype=np.uint64).reshape(16).copy()
+        self.s_g2 = np.ascontiguousarray(s_g2, dtype=np.uint64).reshape(16).copy()
 
 
 def g1_sum(points):

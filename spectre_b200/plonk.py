@@ -23,6 +23,7 @@ from collections import namedtuple
 import numpy as np
 
 from . import halo2
+from .transcript import EvmTranscriptRead
 
 R_MOD = 0x30644e72e131a029b85045b68181585d2833e84879b9709143e1f593f0000001
 P_MOD = 0x30644e72e131a029b85045b68181585d97816a916871ca8d3c208c16d87cfd47
@@ -1133,3 +1134,242 @@ def check_pk(E, pk, max_rows=16, timings=None):
                     failures.append(KeyFailure(kind, c, rows, total))
         lap("sigma")
     return failures
+
+
+# ---- verifier -----------------------------------------------------------------------------------------------------
+# [UPSTREAM] halo2_proofs/src/plonk/verifier.rs verify_proof with VerifierSHPLONK and SingleStrategy
+# (poly/kzg/multiopen/shplonk/verifier.rs, poly/kzg/strategy.rs): what snark_verifier_sdk::gen_proof runs on every proof it
+# makes. The transcript replay and the quotient identity are host work on a few hundred bytes; the device does the one
+# multiexp per proof (a few dozen terms) and the pairing check, so a batch of proofs is decided by one pairing launch sequence.
+class VerifyingKey(namedtuple("VerifyingKey", "cs k vk_digest fixed_commitments sigma_commitments")):
+    """The part of a proving key a verifier reads: the constraint system, k, the transcript digest and the commitments to the
+    fixed and permutation (sigma) columns, as affine (x, y) ints."""
+
+
+def verifying_key(pk):
+    return VerifyingKey(pk.cs, pk.k, pk.vk_digest, list(pk.fixed_commitments), list(pk.sigma_commitments))
+
+
+class ProofFailure(namedtuple("ProofFailure", "kind detail")):
+    """Why verify_proof rejects a proof. kind "transcript": the proof bytes cannot be read (too short, trailing bytes, a scalar
+    >= r, a point off the curve, or anything else the reading transcript refuses); "opening": the bytes read, but the SHPLONK
+    opening's pairing check fails. detail: a human-readable reason."""
+
+
+def _g1_limbs(pt):
+    return np.frombuffer(_point_bytes(pt), dtype="<u8").astype(np.uint64)
+
+
+def _opening_points(be, vp, vk, instances, proof, transcript_read):
+    """Replay one proof up to the SHPLONK verifier's two G1 points (P1, P2), the opening holding iff
+    e(P1, [1]_2) e(P2, -[s]_2) = 1; a ProofFailure("transcript", ...) when the bytes cannot be read."""
+    cs, k = vk.cs, vk.k
+    n = 1 << k
+    bf = cs.blinding_factors()
+    usable = n - (bf + 1)
+    if len(instances) != cs.num_instance:
+        raise ValueError("verify_proof: %d instance columns given, the circuit has %d (upstream: Error::InvalidInstances)" % (len(instances), cs.num_instance))
+    for col in instances:
+        if len(col) > usable:
+            raise ValueError("verify_proof: an instance column has more than %d values (upstream: Error::InstanceTooLarge)" % usable)
+    if len(vk.fixed_commitments) != cs.num_fixed or len(vk.sigma_commitments) != len(cs.permutation):
+        raise ValueError("verify_proof: the verifying key has %d fixed and %d sigma commitments, the circuit %d and %d"
+                         % (len(vk.fixed_commitments), len(vk.sigma_commitments), cs.num_fixed, len(cs.permutation)))
+    w = omega_of(k)
+    R = R_MOD
+    try:
+        T = transcript_read(vk.vk_digest, bytes(proof))
+
+        def rd(f):
+            v = f()
+            if T.pos > len(T.stream):
+                raise ValueError("the proof ends early (%d bytes)" % len(T.stream))
+            return v
+        pt, sc = lambda: rd(T.read_ec_point), lambda: rd(T.read_scalar)
+        for col in instances:
+            for v in col:
+                T.common_scalar(v)
+        advice_c = [pt() for _ in range(cs.num_advice)]
+        theta = T.squeeze_challenge()
+        permuted_c = [(pt(), pt()) for _ in cs.lookups]
+        beta = T.squeeze_challenge(); gamma = T.squeeze_challenge()
+        chunk = max(1, cs.chunk_len())
+        n_sets = -(-len(cs.permutation) // chunk) if cs.permutation else 0
+        perm_c = [pt() for _ in range(n_sets)]
+        lookz_c = [pt() for _ in cs.lookups]
+        random_c = pt()
+        y = T.squeeze_challenge()
+        h_c = [pt() for _ in range(cs.degree() - 1)]
+        x = T.squeeze_challenge()
+        adv = {q: sc() for q in cs.advice_queries}
+        fix = {q: sc() for q in cs.fixed_queries}
+        random_eval = sc()
+        sigma_evals = [sc() for _ in cs.permutation]
+        perm_evals = []
+        for s in range(n_sets):
+            e0, e1 = sc(), sc()
+            perm_evals.append((e0, e1, sc() if s + 1 < n_sets else None))
+        look_evals = [tuple(sc() for _ in range(5)) for _ in cs.lookups]   # z, z_next, a', a'_inv, s'
+        y2 = T.squeeze_challenge(); v = T.squeeze_challenge()
+        h1 = pt()
+        u = T.squeeze_challenge()
+        h2 = pt()
+        if T.pos != len(T.stream):
+            return ProofFailure("transcript", "%d trailing bytes after the proof" % (len(T.stream) - T.pos))
+    except ValueError as e:
+        return ProofFailure("transcript", str(e))
+
+    # ---- the quotient identity at x: the h(x) the proof must open to --------------------------------------------------
+    xn = pow(x, n, R)
+    inv = lambda a: pow(a % R, -1, R)
+    inst_rots = sorted({r for _, r in cs.instance_queries})
+    max_inst = max([len(c) for c in instances] or [0])
+    rows = set([0, usable] + list(range(usable + 1, n)) + [i - r for r in inst_rots for i in range(max_inst)])
+    L = {i: (xn - 1) * pow(w, i % n, R) % R * inv(n * (x - pow(w, i % n, R))) % R for i in rows}
+    l0, l_last = L[0], L[usable]
+    l_active = (1 - l_last - sum(L[i] for i in range(usable + 1, n))) % R
+    inst = {(c, r): sum(val * L[i - r] for i, val in enumerate(instances[c])) % R for c, r in cs.instance_queries}
+
+    def ev(e):
+        t = e[0]
+        if t == "const": return e[1]
+        if t == "fixed": return fix[(e[1], e[2])]
+        if t == "advice": return adv[(e[1], e[2])]
+        if t == "instance": return inst[(e[1], e[2])]
+        if t == "neg": return -ev(e[1]) % R
+        if t == "sum": return (ev(e[1]) + ev(e[2])) % R
+        if t == "prod": return ev(e[1]) * ev(e[2]) % R
+        if t == "scaled": return ev(e[1]) * e[2] % R
+        raise ValueError("unknown expression node %r" % (t,))
+    acc = 0
+    for g in cs.gates:
+        acc = (acc * y + ev(g)) % R
+    if n_sets:
+        col_eval = lambda kind, c: {"fixed": fix, "advice": adv, "instance": inst}[kind][(c, 0)]
+        acc = (acc * y + l0 * (1 - perm_evals[0][0])) % R
+        zl = perm_evals[-1][0]
+        acc = (acc * y + l_last * (zl * zl - zl)) % R
+        for s in range(1, n_sets):
+            acc = (acc * y + l0 * (perm_evals[s][0] - perm_evals[s - 1][2])) % R
+        for s in range(n_sets):
+            left, right = perm_evals[s][1], perm_evals[s][0]
+            for c in range(s * chunk, min((s + 1) * chunk, len(cs.permutation))):
+                kind, col = cs.permutation[c]
+                left = left * (col_eval(kind, col) + beta * sigma_evals[c] + gamma) % R
+                right = right * (col_eval(kind, col) + beta * x % R * pow(DELTA, c, R) + gamma) % R
+            acc = (acc * y + l_active * (left - right)) % R
+    for (ins, tbs), (z, z_next, a_p, a_inv, s_p) in zip(cs.lookups, look_evals):
+        ci = ct = 0
+        for e in ins: ci = (ci * theta + ev(e)) % R
+        for e in tbs: ct = (ct * theta + ev(e)) % R
+        acc = (acc * y + l0 * (1 - z)) % R
+        acc = (acc * y + l_last * (z * z - z)) % R
+        acc = (acc * y + l_active * (z_next * (a_p + beta) % R * (s_p + gamma) - z * (ci + beta) % R * (ct + gamma))) % R
+        acc = (acc * y + l0 * (a_p - s_p)) % R
+        acc = (acc * y + l_active * (a_p - s_p) % R * (a_p - a_inv)) % R
+    expected_h = acc * inv(xn - 1) % R
+
+    # ---- SHPLONK: the queries in create_proof's order, one linear combination of commitments per opening ------------
+    xw = lambda r: x * pow(w, r % n, R) % R
+    q, commits = [], {}
+
+    def query(pid, terms, point, value):
+        commits[pid] = terms                                  # terms: [(scalar, point)] summing to the polynomial's commitment
+        q.append((pid, point, value))
+    for (c, r) in cs.advice_queries: query(("advice", c), [(1, advice_c[c])], xw(r), adv[(c, r)])
+    for s, (e0, e1, _) in enumerate(perm_evals):
+        query(("perm", s), [(1, perm_c[s])], x, e0); query(("perm", s), [(1, perm_c[s])], xw(1), e1)
+    for s in reversed(range(n_sets - 1)):
+        query(("perm", s), [(1, perm_c[s])], xw(-(bf + 1)), perm_evals[s][2])
+    for li, (z, z_next, a_p, a_inv, s_p) in enumerate(look_evals):
+        pin, ptab = permuted_c[li]
+        query(("lk_z", li), [(1, lookz_c[li])], x, z); query(("lk_a", li), [(1, pin)], x, a_p); query(("lk_s", li), [(1, ptab)], x, s_p)
+        query(("lk_a", li), [(1, pin)], xw(-1), a_inv); query(("lk_z", li), [(1, lookz_c[li])], xw(1), z_next)
+    for (c, r) in cs.fixed_queries: query(("fixed", c), [(1, vk.fixed_commitments[c])], xw(r), fix[(c, r)])
+    for c, e in enumerate(sigma_evals): query(("sigma", c), [(1, vk.sigma_commitments[c])], x, e)
+    query(("h",), [(pow(xn, i, R), hc) for i, hc in enumerate(h_c)], x, expected_h)       # h(X) = sum_i X^(n i) h_i(X)
+    query(("random",), [(1, random_c)], x, random_eval)
+    sets = rotation_sets(q)
+    super_pts = []
+    for pts, _, _ in sets:
+        for p in pts:
+            if p not in super_pts: super_pts.append(p)
+
+    def interp_eval(pts, evs, at):                            # the interpolation of (pts, evs) evaluated at `at`
+        tot = 0
+        for j, (pj, ej) in enumerate(zip(pts, evs)):
+            num = den = 1
+            for m, pm in enumerate(pts):
+                if m != j:
+                    num = num * (at - pm) % R; den = den * (pj - pm) % R
+            tot = (tot + ej * num % R * inv(den)) % R
+        return tot
+    # P1 = (sum_ij v^i Z_{T\S_i}(u) y^j (C_ij - r_ij(u) G) - Z_T(u) h1) / Z_{T\S_0}(u) + u h2, P2 = h2:
+    # the opening holds iff P1 = s h2, i.e. e(P1, [1]_2) e(P2, -[s]_2) = 1
+    terms, const, z0 = {}, 0, None
+    for i, (pts, pids, evs) in enumerate(sets):
+        zi = 1
+        for p in super_pts:
+            if p not in pts: zi = zi * (u - p) % R
+        if i == 0: z0 = zi
+        outer = pow(v, i, R) * zi % R
+        for j, pid in enumerate(pids):
+            wij = outer * pow(y2, j, R) % R
+            for s_, c in commits[pid]:
+                terms[c] = (terms.get(c, 0) + wij * s_) % R
+            const = (const + wij * interp_eval(pts, evs[j], u)) % R
+    zt = 1
+    for p in super_pts: zt = zt * (u - p) % R
+    z0_inv = inv(z0)
+    g = _point_from(vp.g.tobytes())
+    terms[g] = (terms.get(g, 0) - const) % R
+    terms[h1] = (terms.get(h1, 0) - zt) % R
+    bases = [c for c in terms]
+    scalars = [terms[c] * z0_inv % R for c in bases]
+    bases.append(h2); scalars.append(u)
+    p1 = halo2.jacobian_to_affine_ints(be.best_multiexp(fr_mont_rows(scalars), np.stack([_g1_limbs(c) for c in bases])))
+    return p1, h2
+
+
+def _neg_g2(q):
+    """-Q for a G2 affine point as uint64[16] Montgomery limbs (x.c0, x.c1, y.c0, y.c1): both y coordinates negated mod p"""
+    out = np.array(q, dtype=np.uint64).reshape(4, 4).copy()
+    for c in (2, 3):
+        v = int(out[c, 0]) | int(out[c, 1]) << 64 | int(out[c, 2]) << 128 | int(out[c, 3]) << 192
+        v = (P_MOD - v) % P_MOD
+        out[c] = [(v >> (64 * j)) & 0xFFFFFFFFFFFFFFFF for j in range(4)]
+    return out.reshape(16)
+
+
+def verify_proofs(be, vp, items, transcript_read=EvmTranscriptRead):
+    """verify_proof for every (vk, instances, proof) of `items`; the keys may differ (step and committee-update proofs together).
+    One verdict per item, in verify_proof's form: None for an accepted proof, else a ProofFailure. Every proof that gets past
+    its transcript costs one multiexp, and all of them are decided by ONE pairing_check_batch call of m = 2 pairs per check.
+    be: anything with best_multiexp(coeffs, bases) and pairing_check_batch(ps, qs, m) in the layouts of halo2.Backend; vp: a
+    halo2.ParamsVerifierKZG."""
+    verdicts, todo, ps, qs = [], [], [], []
+    neg_s_g2 = _neg_g2(vp.s_g2)
+    for vk, instances, proof in items:
+        got = _opening_points(be, vp, vk, instances, proof, transcript_read)
+        if isinstance(got, ProofFailure):
+            verdicts.append(got)
+            continue
+        verdicts.append(None)
+        todo.append(len(verdicts) - 1)
+        p1, p2 = got
+        ps += [_g1_limbs(p1), _g1_limbs(p2)]
+        qs += [vp.g2, neg_s_g2]
+    if todo:
+        ok = be.pairing_check_batch(np.stack(ps), np.stack(qs), 2)
+        for i, good in zip(todo, ok):
+            if not good:
+                verdicts[i] = ProofFailure("opening", "the SHPLONK opening fails its pairing check")
+    return verdicts
+
+
+def verify_proof(be, vp, vk, instances, proof, transcript_read=EvmTranscriptRead):
+    """halo2_proofs::plonk::verify_proof with VerifierSHPLONK and SingleStrategy: None when the proof is accepted, else a
+    ProofFailure. instances: per instance column a list of ints (a wrong column count raises ValueError, a caller error as
+    upstream's Error::InvalidInstances). transcript_read: EvmTranscriptRead (default) or poseidon.PoseidonTranscriptRead, the
+    reading side of the transcript create_proof wrote. The final check is one pairing_check_batch call of one check."""
+    return verify_proofs(be, vp, [(vk, instances, proof)], transcript_read)[0]
