@@ -1136,6 +1136,157 @@ def check_pk(E, pk, max_rows=16, timings=None):
     return failures
 
 
+# ---- params check -------------------------------------------------------------------------------------------------
+class ParamsFailure(namedtuple("ParamsFailure", "kind index detail")):
+    """One failing part of a ParamsKZG (check_params). kind and index:
+      "g_generator" (0): g[0] is not the G1 generator (1, 2), or is not vp.g;
+      "g2_generator" (0): vp.g2 is not halo2curves' G2 generator;
+      "trailer" (0 g2, 1 s_g2): the handle's own G2 trailer differs from the vp given;
+      "s_g2" (0): the pairing refuses vp.s_g2 (off the curve or outside the G2 subgroup), detail = the library's error text;
+      "powers" (j): the smallest j >= 1 with g[j] != s g[j - 1] for the s of vp.s_g2;
+      "lagrange" (i): the smallest i with g_lagrange[i] != g_to_lagrange(g)[i], g as stored.
+    detail: a human-readable reason."""
+
+
+PARAMS_FAILURE_KINDS = ("g_generator", "g2_generator", "trailer", "s_g2", "powers", "lagrange")
+
+# halo2curves' G2Affine::generator (EIP-197): ((x.c0, x.c1), (y.c0, y.c1))
+G2_GENERATOR = ((0x1800deef121f1e76426a00665e5c4479674322d4f75edadd46debd5cd992f6ed, 0x198e9393920d483a7260bfb731fb5d25f1aa493335a9e71297e485b7aef312c2),
+                (0x12c85ea5db8c6deb4aab71808dcb408fe3d1e7690c43d37b4ce6cc0166fa7daa, 0x090689d0585ff075ec9e99ad690c3395bc4b313370b38ef355acdadcd122975b))
+
+
+def _g2_limbs(q):
+    """G2 affine ((x.c0, x.c1), (y.c0, y.c1)) ints -> uint64[16] Montgomery limbs in the params trailer's order"""
+    return np.frombuffer(b"".join((v * _FQ_MONT % P_MOD).to_bytes(32, "little") for c in q for v in c), dtype="<u8").astype(np.uint64)
+
+
+def check_params(E, be, vp=None, seed=None, timings=None):
+    """Check that the points of the engine's params fit together: a list of ParamsFailure in the order of PARAMS_FAILURE_KINDS,
+    [] for sound params. E: an engine bound to the params (E.params, E.k == params.k); be: anything with pairing_check_batch(ps,
+    qs, m) in halo2.Backend's layouts, whose refusal of an input raises halo2.BackendError; vp: the halo2.ParamsVerifierKZG the
+    proofs will be verified against (a verifier contract's constants, say), by default params.verifier_params(); seed: 32 bytes
+    for the ChaCha20 draws (default os.urandom(32)), the same seed giving the same report. A handle without a 2^k SRS and its
+    g_lagrange (from_bases) raises ValueError. Nothing is written to the params, and every temporary is freed before it returns.
+
+    Every n-row vector stays on the engine: the draws, their inverse NTT and the MSMs, which go through the window tables of a
+    handle that has them. Only points and verdicts reach the host.
+      * powers: with r drawn at random, A = sum_{i<m} r_i g[i] and B = sum_{i<m} r_i g[i+1] (two prefix MSMs over one draw). The
+        chain g[j] = s g[j-1] holds for every j <= m exactly when B = s A, decided by one pairing check e(B, g2) e(A, -s_g2) = 1.
+        m = n - 1 first; if it fails, a bisection over m with fresh draws per step (ceil(log2 n) more checks) finds the first j.
+        When the pairing refuses vp.s_g2 (reported as s_g2) or vp.g2 (reported as g2_generator), powers is not checked.
+      * lagrange: with v drawn at random and c = lagrange_to_coeff(v), MSM(v, g_lagrange) = MSM(c, g) holds exactly when
+        g_lagrange = g_to_lagrange(g) (the basis downsize computes from g). No pairing. If it fails, a bisection with v zeroed
+        past m, one inverse NTT and one full MSM over g per step, finds the first row.
+    Soundness: G1 has prime order r, so a wrong prefix passes one check with probability at most 1/r over the draws. The checks
+    are random linear combinations: they cannot count failures, so each kind reports its first failure only.
+    timings: a dict that gets the wall time of the stages points / powers / lagrange."""
+    import os
+    import time
+    params = E.params
+    if E.k != params.k:
+        raise ValueError("check_params: the engine is for k = %d, the params for k = %d" % (E.k, params.k))
+    n = 1 << params.k
+    G, GL = halo2.BASIS_G, halo2.BASIS_G_LAGRANGE
+    refused = "check_params: the handle holds no 2^k SRS with its g_lagrange (from_bases bases are not params)"
+    if params.n != n:
+        raise ValueError(refused)
+    try:
+        params.get_g(0, 1, basis=GL)
+    except halo2.BackendError:
+        raise ValueError(refused) from None
+    g0 = params.get_g(0, 1)[0]
+    own_g2, own_s_g2 = params.get_g2()
+    has_trailer = own_g2.any() and own_s_g2.any()
+    given = vp is not None
+    vp = params.verifier_params() if vp is None else vp
+    seed = os.urandom(32) if seed is None else seed
+    t_last = [time.perf_counter()]
+
+    def lap(name):
+        if timings is not None:
+            E.sync(); t = time.perf_counter(); timings[name] = timings.get(name, 0.0) + t - t_last[0]; t_last[0] = t
+    drawn = [0]
+
+    def draw(rows):
+        """fresh draws: each call takes the next `rows` elements of the seed's stream"""
+        drawn[0] += rows
+        return E.random_chacha(seed, drawn[0] - rows, rows)
+
+    # ---- points: the generators and the trailer, on the host --------------------------------------------------------
+    failures = []
+    generator = _g1_limbs((1, 2))
+    if not np.array_equal(g0, generator) or not np.array_equal(g0, vp.g):
+        failures.append(ParamsFailure("g_generator", 0, "g[0] is %s, the G1 generator is (1, 2) and vp.g is %s"
+                                      % (_point_from(g0.tobytes()), _point_from(vp.g.tobytes()))))
+    g2_ok = np.array_equal(vp.g2, _g2_limbs(G2_GENERATOR))
+    if not g2_ok:
+        failures.append(ParamsFailure("g2_generator", 0, "vp.g2 is not the G2 generator"))
+    if given and has_trailer:
+        for i, (own, want) in enumerate(((own_g2, vp.g2), (own_s_g2, vp.s_g2))):
+            if not np.array_equal(own, want):
+                failures.append(ParamsFailure("trailer", i, "the params' own %s differs from vp's" % ("g2", "s_g2")[i]))
+                break
+    lap("points")
+
+    # ---- powers: g[j] = s g[j-1] -----------------------------------------------------------------------------------
+    neg_s_g2 = _neg_g2(vp.s_g2)
+
+    def chain_holds(m):
+        """g[j] = s g[j-1] for 1 <= j <= m: d = (0, r_0 .. r_{m-1}, 0), A = MSM(d[1:m+2]) and B = MSM(d[0:m+1]) over g[0..m]"""
+        d = draw(m + 2)
+        E.zero(E.view(d, 0, 1)); E.zero(E.view(d, m + 1, m + 2))
+        a, b = E.commit(G, [E.view(d, 1, m + 2), E.view(d, 0, m + 1)], m + 1)
+        del d
+        return be.pairing_check_batch(np.stack([_g1_limbs(b), _g1_limbs(a)]), np.stack([vp.g2, neg_s_g2]), 2)[0]
+    if n > 1:
+        try:
+            whole = chain_holds(n - 1)
+        except halo2.BackendError as error:                 # a trailer point refused: find out whether it is s_g2
+            whole = None
+            try:
+                be.pairing_check_batch(np.zeros((1, 8), dtype=np.uint64), vp.s_g2.reshape(1, 16), 1)
+            except halo2.BackendError as e:
+                failures.append(ParamsFailure("s_g2", 0, str(e)))
+            else:
+                if g2_ok:                                   # the generator and s_g2 both pass: not a verdict on the points
+                    raise error
+                # else vp.g2 was refused, and g2_generator already names it
+        if whole is False:
+            lo, hi = 0, n - 1                               # the chain holds up to lo and breaks by hi
+            while hi - lo > 1:
+                mid = (lo + hi) // 2
+                if chain_holds(mid):
+                    lo = mid
+                else:
+                    hi = mid
+            failures.append(ParamsFailure("powers", hi, "g[%d] is not s g[%d]" % (hi, hi - 1)))
+    lap("powers")
+
+    # ---- lagrange: g_lagrange = g_to_lagrange(g) -------------------------------------------------------------------
+    def rows_hold(m):
+        """g_lagrange[i] = g_to_lagrange(g)[i] for i < m: v zeroed past m, MSM(v, g_lagrange) = MSM(lagrange_to_coeff(v), g)"""
+        v = draw(n)
+        if m < n:
+            E.zero(E.view(v, m, n))
+        c = E.clone(v)
+        E.lagrange_to_coeff(c)
+        lhs = E.commit(GL, [v], m)[0]
+        del v
+        rhs = E.commit(G, [c], n)[0]
+        return tuple(lhs) == tuple(rhs)
+    if not rows_hold(n):
+        lo, hi = 0, n                                       # rows < lo agree, some row < hi does not
+        while hi - lo > 1:
+            mid = (lo + hi) // 2
+            if rows_hold(mid):
+                lo = mid
+            else:
+                hi = mid
+        failures.append(ParamsFailure("lagrange", hi - 1, "g_lagrange[%d] is not row %d of g_to_lagrange(g)" % (hi - 1, hi - 1)))
+    lap("lagrange")
+    return failures
+
+
 # ---- verifier -----------------------------------------------------------------------------------------------------
 # [UPSTREAM] halo2_proofs/src/plonk/verifier.rs verify_proof with VerifierSHPLONK and SingleStrategy
 # (poly/kzg/multiopen/shplonk/verifier.rs, poly/kzg/strategy.rs): what snark_verifier_sdk::gen_proof runs on every proof it
