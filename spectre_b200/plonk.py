@@ -22,8 +22,8 @@ from collections import namedtuple
 
 import numpy as np
 
-from . import halo2
-from .transcript import EvmTranscriptRead
+from . import halo2, poseidon
+from .transcript import EvmTranscriptRead, keccak256
 
 R_MOD = 0x30644e72e131a029b85045b68181585d2833e84879b9709143e1f593f0000001
 P_MOD = 0x30644e72e131a029b85045b68181585d97816a916871ca8d3c208c16d87cfd47
@@ -1304,16 +1304,34 @@ def verifying_key(pk):
 class ProofFailure(namedtuple("ProofFailure", "kind detail")):
     """Why verify_proof rejects a proof. kind "transcript": the proof bytes cannot be read (too short, trailing bytes, a scalar
     >= r, a point off the curve, or anything else the reading transcript refuses); "opening": the bytes read, but the SHPLONK
-    opening's pairing check fails. detail: a human-readable reason."""
+    opening's pairing check fails. With accumulator indices (an aggregation proof, checked as its verifier contract does) two
+    more: "accumulator_encoding": the 12 instance limbs of the KZG accumulator do not decode to two curve points
+    (accumulator_from_limbs), decided on the host; "accumulator": they decode, but e(lhs, [1]_2) e(rhs, -[s]_2) != 1, so the
+    inner snark the accumulator stands for is invalid. The first failure in the order transcript, accumulator_encoding,
+    opening, accumulator is reported. detail: a human-readable reason."""
 
 
 def _g1_limbs(pt):
     return np.frombuffer(_point_bytes(pt), dtype="<u8").astype(np.uint64)
 
 
+def _multiexp(be, scalars, points):
+    """sum_i scalars[i] points[i] on the backend, for ints and affine int points; the identity is (0, 0)"""
+    return halo2.jacobian_to_affine_ints(be.best_multiexp(fr_mont_rows(scalars), np.stack([_g1_limbs(c) for c in points])))
+
+
 def _opening_points(be, vp, vk, instances, proof, transcript_read):
     """Replay one proof up to the SHPLONK verifier's two G1 points (P1, P2), the opening holding iff
     e(P1, [1]_2) e(P2, -[s]_2) = 1; a ProofFailure("transcript", ...) when the bytes cannot be read."""
+    got = _opening_terms(vp, vk, instances, proof, transcript_read)
+    if isinstance(got, ProofFailure):
+        return got
+    scalars, bases, h2 = got
+    return _multiexp(be, scalars, bases), h2
+
+
+def _opening_terms(vp, vk, instances, proof, transcript_read):
+    """The host part of _opening_points: (scalars, bases, P2) with P1 = sum_i scalars[i] bases[i], or the ProofFailure"""
     cs, k = vk.cs, vk.k
     n = 1 << k
     bf = cs.blinding_factors()
@@ -1478,8 +1496,7 @@ def _opening_points(be, vp, vk, instances, proof, transcript_read):
     bases = [c for c in terms]
     scalars = [terms[c] * z0_inv % R for c in bases]
     bases.append(h2); scalars.append(u)
-    p1 = halo2.jacobian_to_affine_ints(be.best_multiexp(fr_mont_rows(scalars), np.stack([_g1_limbs(c) for c in bases])))
-    return p1, h2
+    return scalars, bases, h2
 
 
 def _neg_g2(q):
@@ -1492,35 +1509,170 @@ def _neg_g2(q):
     return out.reshape(16)
 
 
-def verify_proofs(be, vp, items, transcript_read=EvmTranscriptRead):
+# ---- the KZG accumulator of an aggregation proof ----------------------------------------------------------------------
+# [UPSTREAM] snark-verifier's KzgAccumulator and KzgAs (pcs/kzg/accumulation.rs), and what the verifier contract its EVM
+# loader generates does with the accumulator (contracts/snark-verifiers/sync_step_verifier.sol:213-236 decodes it,
+# :1165-1208 folds it into the final pairing; committee_update_verifier.sol:214-237 and :1178-1221 alike). An aggregation
+# circuit verifies its inner snark up to the pairing and exposes what is left, a pair (lhs, rhs) with the inner snark valid
+# iff e(lhs, [1]_2) = e(rhs, [s]_2), as 12 public instances; that pairing is the outer proof's verifier's job.
+class KzgAccumulator(namedtuple("KzgAccumulator", "lhs rhs")):
+    """A KZG accumulator: two affine G1 points as (x, y) ints, valid iff e(lhs, [1]_2) e(rhs, -[s]_2) = 1."""
+
+
+ACCUMULATOR_LIMBS, ACCUMULATOR_LIMB_BITS = 3, 88
+# (column, row) of the 12 accumulator limbs among the instances, as snark-verifier's accumulator_indices: Spectre's
+# aggregation circuits put them first in their one instance column
+AGGREGATION_ACCUMULATOR_INDICES = [(0, i) for i in range(4 * ACCUMULATOR_LIMBS)]
+_M256 = (1 << 256) - 1
+
+
+def accumulator_to_limbs(acc):
+    """The 12 instance words of a KzgAccumulator: lhs.x, lhs.y, rhs.x, rhs.y, each as three 88-bit limbs, least significant first."""
+    mask = (1 << ACCUMULATOR_LIMB_BITS) - 1
+    return [(v >> (ACCUMULATOR_LIMB_BITS * i)) & mask for v in (acc.lhs[0], acc.lhs[1], acc.rhs[0], acc.rhs[1])
+            for i in range(ACCUMULATOR_LIMBS)]
+
+
+def accumulator_from_limbs(words):
+    """The KzgAccumulator that 12 instance words encode, decoded exactly as the generated verifier contract decodes it, or None
+    where the contract refuses it. Each word is first reduced mod r (the contract reads every instance as mod(calldataload, f_q));
+    a coordinate is l0 + l1 2^88 + l2 2^176 with the EVM's wrap-around mod 2^256, so limbs of 88 bits or more overlap and are
+    not refused; each point must pass validate_ec_point: x < p, y < p and y^2 = x^3 + 3, which refuses the identity (0, 0)."""
+    words = [int(w) % R_MOD for w in words]
+    if len(words) != 4 * ACCUMULATOR_LIMBS:
+        raise ValueError("accumulator_from_limbs: %d words, an accumulator has %d" % (len(words), 4 * ACCUMULATOR_LIMBS))
+    coords = []
+    for c in range(4):
+        v = 0
+        for i, limb in enumerate(words[ACCUMULATOR_LIMBS * c:ACCUMULATOR_LIMBS * (c + 1)]):
+            v = (v + (limb << (ACCUMULATOR_LIMB_BITS * i))) & _M256
+        coords.append(v)
+    pts = [(coords[0], coords[1]), (coords[2], coords[3])]
+    for x, y in pts:
+        if x >= P_MOD or y >= P_MOD or (y * y - x * x * x - 3) % P_MOD:
+            return None
+    return KzgAccumulator(*pts)
+
+
+def _accumulator_words(instances, indices):
+    indices = list(indices)
+    if len(indices) != 4 * ACCUMULATOR_LIMBS:
+        raise ValueError("accumulator_indices: %d given, an accumulator has %d limbs" % (len(indices), 4 * ACCUMULATOR_LIMBS))
+    words = []
+    for col, row in indices:
+        if not (0 <= col < len(instances) and 0 <= row < len(instances[col])):
+            raise ValueError("accumulator_indices: (%d, %d) is outside the instances" % (col, row))
+        words.append(instances[col][row])
+    return words
+
+
+def _replay(be, vp, vk, instances, proof, transcript_read, indices):
+    """(P1, P2, the decoded accumulator or None without indices), or the first ProofFailure: transcript, then
+    accumulator_encoding, both found on the host before the one multiexp"""
+    words = None if indices is None else _accumulator_words(instances, indices)
+    got = _opening_terms(vp, vk, instances, proof, transcript_read)
+    if isinstance(got, ProofFailure):
+        return got
+    acc = None
+    if words is not None:
+        acc = accumulator_from_limbs(words)
+        if acc is None:
+            return ProofFailure("accumulator_encoding", "the accumulator limbs in the instances are not two points on the curve")
+    scalars, bases, h2 = got
+    return _multiexp(be, scalars, bases), h2, acc
+
+
+def succinct_verify(be, vp, vk, instances, proof, transcript_read=EvmTranscriptRead):
+    """The accumulator a proof leaves for its aggregation: verify_proof without the final pairing (snark-verifier's succinct
+    SHPLONK verifier). KzgAccumulator(P1, P2), which passes the pairing iff the proof's opening holds; for a valid proof it is
+    (s W', W') with W' the proof's last point, the pair every correct SHPLONK verifier reaches. A ProofFailure("transcript", ...)
+    when the bytes cannot be read. Spectre's inner snarks are written with poseidon.PoseidonTranscriptWrite, so pass
+    transcript_read=poseidon.PoseidonTranscriptRead for them. One multiexp on be."""
+    got = _opening_points(be, vp, vk, instances, proof, transcript_read)
+    return got if isinstance(got, ProofFailure) else KzgAccumulator(*got)
+
+
+def aggregate_accumulators(be, accs, transcript=None):
+    """snark-verifier's KzgAs::create_proof as snark_verifier_sdk's aggregation calls it, without zk. One accumulator is
+    returned as it is, whatever the transcript: that is Spectre's case, where each aggregation circuit wraps one snark. Several
+    are folded into sum_i r^i accs[i], starting at r^0 = 1, with one multiexp per side; the result passes the pairing iff every
+    input does, except with probability at most len(accs) / r. r is squeezed from `transcript` (default
+    poseidon.PoseidonTranscriptWrite(0)) after it absorbs each lhs and rhs, in order, as common points.
+    That framing is not pinned against snark-verifier, as poseidon.py's framing is not: snark-verifier squeezes r from the
+    aggregation proof's own Poseidon transcript, which starts without the key digest this default absorbs. So for several
+    accumulators r and the folded pair are this library's own."""
+    accs = [KzgAccumulator(*a) for a in accs]
+    if not accs:
+        raise ValueError("aggregate_accumulators: no accumulator given")
+    if len(accs) == 1:
+        return accs[0]
+    if transcript is None:
+        transcript = poseidon.PoseidonTranscriptWrite(0)
+    for a in accs:
+        transcript.common_ec_point(a.lhs)
+        transcript.common_ec_point(a.rhs)
+    r = transcript.squeeze_challenge()
+    powers = [pow(r, i, R_MOD) for i in range(len(accs))]
+    return KzgAccumulator(_multiexp(be, powers, [a.lhs for a in accs]), _multiexp(be, powers, [a.rhs for a in accs]))
+
+
+def evm_pairing_points(be, vp, vk, instances, proof, accumulator_indices):
+    """The two G1 points the generated verifier contract hands to the pairing precompile (0x08) for an aggregation proof over
+    the EVM transcript, with the r that combines them: (r, P1 + r lhs, P2 + r rhs). (P1, P2) are the SHPLONK opening's points,
+    (lhs, rhs) the accumulator decoded from the instances at accumulator_indices, and r = keccak256(P1 || P2 || lhs || rhs)
+    mod r_F over the 32-byte big-endian coordinates. The contract accepts iff e(P1 + r lhs, [1]_2) e(P2 + r rhs, -[s]_2) = 1,
+    so this reproduces its decision before a transaction is sent. A ProofFailure ("transcript" or "accumulator_encoding")
+    where the contract reverts before it gets that far. Three multiexps on be."""
+    got = _replay(be, vp, vk, instances, proof, EvmTranscriptRead, accumulator_indices)
+    if isinstance(got, ProofFailure):
+        return got
+    p1, p2, acc = got
+    r = int.from_bytes(keccak256(b"".join(v.to_bytes(32, "big") for pt in (p1, p2, acc.lhs, acc.rhs) for v in pt)), "big") % R_MOD
+    return r, _multiexp(be, [1, r], [p1, acc.lhs]), _multiexp(be, [1, r], [p2, acc.rhs])
+
+
+_CHECK_FAILED = {"opening": "the SHPLONK opening fails its pairing check",
+                 "accumulator": "the KZG accumulator in the instances fails its pairing check"}
+
+
+def verify_proofs(be, vp, items, transcript_read=EvmTranscriptRead, accumulator_indices=None):
     """verify_proof for every (vk, instances, proof) of `items`; the keys may differ (step and committee-update proofs together).
-    One verdict per item, in verify_proof's form: None for an accepted proof, else a ProofFailure. Every proof that gets past
-    its transcript costs one multiexp, and all of them are decided by ONE pairing_check_batch call of m = 2 pairs per check.
+    One verdict per item, in verify_proof's form: None for an accepted proof, else a ProofFailure. An item may carry a fourth
+    element, its accumulator indices, which then stand in for `accumulator_indices`: step and aggregation proofs share a batch.
+    Every proof that gets past its transcript and accumulator encoding costs one multiexp, and all of them are decided by ONE
+    pairing_check_batch call of m = 2 pairs per check: one check per proof, and a second for each aggregation proof.
     be: anything with best_multiexp(coeffs, bases) and pairing_check_batch(ps, qs, m) in the layouts of halo2.Backend; vp: a
     halo2.ParamsVerifierKZG."""
     verdicts, todo, ps, qs = [], [], [], []
     neg_s_g2 = _neg_g2(vp.s_g2)
-    for vk, instances, proof in items:
-        got = _opening_points(be, vp, vk, instances, proof, transcript_read)
+    for item in items:
+        vk, instances, proof = item[:3]
+        indices = item[3] if len(item) > 3 else accumulator_indices
+        got = _replay(be, vp, vk, instances, proof, transcript_read, indices)
         if isinstance(got, ProofFailure):
             verdicts.append(got)
             continue
         verdicts.append(None)
-        todo.append(len(verdicts) - 1)
-        p1, p2 = got
-        ps += [_g1_limbs(p1), _g1_limbs(p2)]
-        qs += [vp.g2, neg_s_g2]
+        p1, p2, acc = got
+        checks = [("opening", p1, p2)] + ([] if acc is None else [("accumulator", acc.lhs, acc.rhs)])
+        for kind, a, b in checks:
+            todo.append((len(verdicts) - 1, kind))
+            ps += [_g1_limbs(a), _g1_limbs(b)]
+            qs += [vp.g2, neg_s_g2]
     if todo:
         ok = be.pairing_check_batch(np.stack(ps), np.stack(qs), 2)
-        for i, good in zip(todo, ok):
-            if not good:
-                verdicts[i] = ProofFailure("opening", "the SHPLONK opening fails its pairing check")
+        for (i, kind), good in zip(todo, ok):
+            if not good and verdicts[i] is None:               # the opening's check comes first: the first failure is reported
+                verdicts[i] = ProofFailure(kind, _CHECK_FAILED[kind])
     return verdicts
 
 
-def verify_proof(be, vp, vk, instances, proof, transcript_read=EvmTranscriptRead):
+def verify_proof(be, vp, vk, instances, proof, transcript_read=EvmTranscriptRead, accumulator_indices=None):
     """halo2_proofs::plonk::verify_proof with VerifierSHPLONK and SingleStrategy: None when the proof is accepted, else a
     ProofFailure. instances: per instance column a list of ints (a wrong column count raises ValueError, a caller error as
     upstream's Error::InvalidInstances). transcript_read: EvmTranscriptRead (default) or poseidon.PoseidonTranscriptRead, the
-    reading side of the transcript create_proof wrote. The final check is one pairing_check_batch call of one check."""
-    return verify_proofs(be, vp, [(vk, instances, proof)], transcript_read)[0]
+    reading side of the transcript create_proof wrote. The final check is one pairing_check_batch call of one check.
+    accumulator_indices: for an aggregation proof (AGGREGATION_ACCUMULATOR_INDICES for Spectre's), also decide the KZG
+    accumulator in its instances as the verifier contract does, in the same pairing call; indices outside the instances raise
+    ValueError. None (default) checks the proof alone, as halo2's verify_proof does."""
+    return verify_proofs(be, vp, [(vk, instances, proof)], transcript_read, accumulator_indices)[0]

@@ -26,6 +26,7 @@ from tests.plonk_oracle_engine import OracleEngine, SeededRng  # noqa: E402
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "tests", "golden")
 SEED, GROUPS = 23, 2000
+ACCUMULATOR_SCALAR = 0xACC                  # rhs = ACCUMULATOR_SCALAR * G of the fixtures' accumulator
 # K -> (contract, lookup bits of its range table, number of public inputs): config/sync_step_verifier_23.json,
 # config/committee_update_verifier_24.json (SURVEY.md section 8 rows 4 and 5)
 CONTRACTS = {23: ("sync_step_verifier", 19, "range_table_commit_k23_bits19"), 24: ("committee_update_verifier", 23, "range_table_commit_k24_bits23")}
@@ -35,18 +36,14 @@ def accumulator_limbs(tau, s):
     """12 instance words: (lhs.x, lhs.y, rhs.x, rhs.y) in three 88-bit limbs each, with lhs = tau * rhs -- a valid KZG
     accumulator for the seed-0 SRS, the form the aggregation circuit exposes (sync_step_verifier.sol:213-236)."""
     rhs = pyref.ec_mul((1, 2), s)
-    lhs = pyref.ec_mul(rhs, tau)
-    out = []
-    for v in (lhs[0], lhs[1], rhs[0], rhs[1]):
-        out += [v & ((1 << 88) - 1), (v >> 88) & ((1 << 88) - 1), v >> 176]
-    return out
+    return plonk.accumulator_to_limbs(plonk.KzgAccumulator(pyref.ec_mul(rhs, tau), rhs))
 
 
 def inputs(k, kats):
     contract, bits, _ = CONTRACTS.get(k, ("sync_step_verifier", min(19, k - 2), None))
     sched = kats["transcript_schedule"][contract]
     tau = orc.fr_ints(orc.srs_tau().reshape(1, 4))[0]
-    instances = accumulator_limbs(tau, 0xACC) + [0x5eed0001 + i for i in range(sched["num_instances"] - 12)]
+    instances = accumulator_limbs(tau, ACCUMULATOR_SCALAR) + [0x5eed0001 + i for i in range(sched["num_instances"] - 12)]
     cs = plonk_circuits.aggregation_shape()
     fixed, adv, copies = plonk_circuits.aggregation_witness(cs, k, instances, bits, GROUPS, seed=SEED)
     return cs, tau, instances, fixed, adv, copies, int(sched["vk_digest"]), bits
