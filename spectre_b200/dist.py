@@ -4,6 +4,7 @@ reduction op). Backend-agnostic (`nccl` on the GPU box, `gloo` in the CPU tests)
 import numpy as np
 
 from . import halo2
+from .halo2 import MONT_RADIX, R_MOD
 
 
 def shard_range(n, rank, world):
@@ -27,8 +28,7 @@ def fold_partials(partials, world, device=None, group=None):
     return halo2.g1_sum_batch(allp)                                 # one host call for the whole batch
 
 
-R_MOD = 0x30644e72e131a029b85045b68181585d2833e84879b9709143e1f593f0000001
-_MONT = (1 << 256) % R_MOD
+_MONT = MONT_RADIX % R_MOD
 
 
 def _mont_int(a):

@@ -28,6 +28,20 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("SPB_LIB_PATH") or os.path.join(_HERE, "libspectre_b200.so")   # SPB_LIB_PATH: A/B builds (tools/), never the product default
 
+# BN254: r is the order of G1 and the modulus of the scalar field Fr, p the modulus of the base field Fq, and G1 is
+# y^2 = x^3 + 3 over Fq. An element of either field is held as the four little-endian 64-bit limbs of its Montgomery form
+# a 2^256 mod the modulus.
+R_MOD = 0x30644e72e131a029b85045b68181585d2833e84879b9709143e1f593f0000001
+P_MOD = 0x30644e72e131a029b85045b68181585d97816a916871ca8d3c208c16d87cfd47
+MONT_RADIX = 1 << 256
+FQ_MONT_INV = pow(MONT_RADIX, -1, P_MOD)
+
+
+def g1_on_curve(x, y):
+    """x and y are canonical Fq ints (below p) and (x, y) lies on y^2 = x^3 + 3; the identity (0, 0) does not"""
+    return x < P_MOD and y < P_MOD and (y * y - x * x * x - 3) % P_MOD == 0
+
+
 BASIS_G = 0
 BASIS_G_LAGRANGE = 1
 
@@ -762,12 +776,11 @@ def g1_sum_batch(points):
     return out
 
 
-def jacobian_to_affine_ints(j, p_mod=0x30644e72e131a029b85045b68181585d97816a916871ca8d3c208c16d87cfd47):
+def jacobian_to_affine_ints(j):
     """(12,) Jacobian Montgomery limbs -> (x, y) canonical ints, identity -> (0, 0). Pure Python (for tests/logs)."""
     j = np.ascontiguousarray(j, dtype=np.uint64).reshape(3, 4)
-    rinv = pow(1 << 256, -1, p_mod)
-    v = [(int(r[0]) | int(r[1]) << 64 | int(r[2]) << 128 | int(r[3]) << 192) * rinv % p_mod for r in j]
+    v = [(int(r[0]) | int(r[1]) << 64 | int(r[2]) << 128 | int(r[3]) << 192) * FQ_MONT_INV % P_MOD for r in j]
     if v[2] == 0:
         return (0, 0)
-    zi = pow(v[2], -1, p_mod)
-    return (v[0] * zi * zi % p_mod, v[1] * zi * zi * zi % p_mod)
+    zi = pow(v[2], -1, P_MOD)
+    return (v[0] * zi * zi % P_MOD, v[1] * zi * zi * zi % P_MOD)

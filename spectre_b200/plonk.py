@@ -17,17 +17,18 @@ parity tests bind the same driver to the CPU oracle and require byte-identical p
 A circuit is described by a `ConstraintSystem` of expression trees -- the information `pk.get_vk().cs()` holds
 upstream. Expressions are nested tuples built with Const / Fixed / Advice / Instance / Neg / Sum / Prod / Scaled.
 """
+import os
 import secrets
+import time
 from collections import namedtuple
 
 import numpy as np
 
 from . import halo2, poseidon
+from .halo2 import FQ_MONT_INV, MONT_RADIX, P_MOD, R_MOD, g1_on_curve
 from .transcript import EvmTranscriptRead, keccak256
 
-R_MOD = 0x30644e72e131a029b85045b68181585d2833e84879b9709143e1f593f0000001
-P_MOD = 0x30644e72e131a029b85045b68181585d97816a916871ca8d3c208c16d87cfd47
-_MONT = (1 << 256) % R_MOD
+_MONT = MONT_RADIX % R_MOD
 _MONT_INV = pow(_MONT, -1, R_MOD)
 ROOT_OF_UNITY = pow(7, (R_MOD - 1) >> 28, R_MOD)
 DELTA = pow(7, 1 << 28, R_MOD)
@@ -548,17 +549,42 @@ def default_vk_digest(pk):
 # file: like upstream's `ProvingKey::read::<_, ConcreteCircuit>(reader, format, params)` the reader gets it from the circuit.
 # This restates the upstream layout from memory (no Rust toolchain here to diff a real .pkey against it): files written and
 # read by this repo round-trip, byte compatibility with upstream's files is unverified.
-_FQ_MONT = (1 << 256) % P_MOD
+
+# ---- curve points on the host: each Fq coordinate as its Montgomery limbs, 32 little-endian bytes; the G1 identity is
+# (0, 0), a G2 point is ((x.c0, x.c1), (y.c0, y.c1)) -------------------------------------------------------------------------
+_FQ_MONT = MONT_RADIX % P_MOD
 
 
-def _point_bytes(pt):
-    x, y = pt
-    return b"".join(((v * _FQ_MONT) % P_MOD).to_bytes(32, "little") for v in (x, y))
+def _fq_bytes(vals):
+    return b"".join((v * _FQ_MONT % P_MOD).to_bytes(32, "little") for v in vals)
 
 
-def _point_from(raw):
-    inv = pow(_FQ_MONT, -1, P_MOD)
-    return tuple(int.from_bytes(raw[i:i + 32], "little") * inv % P_MOD for i in (0, 32))
+def _fq_int(raw):
+    return int.from_bytes(raw, "little") * FQ_MONT_INV % P_MOD
+
+
+def _limbs(raw):
+    return np.frombuffer(raw, dtype="<u8").astype(np.uint64)
+
+
+def _g1_from(raw):
+    """(x, y) ints of a G1 point given as 64 bytes of limbs"""
+    return _fq_int(raw[:32]), _fq_int(raw[32:64])
+
+
+def _g1_limbs(pt):
+    return _limbs(_fq_bytes(pt))
+
+
+def _g2_limbs(q):
+    """uint64[16] in the params trailer's order x.c0, x.c1, y.c0, y.c1"""
+    return _limbs(_fq_bytes(v for c in q for v in c))
+
+
+def _neg_g2(q):
+    """-Q for a G2 point as uint64[16] limbs: x as given, both y coordinates negated mod p"""
+    raw = np.asarray(q, dtype=np.uint64).reshape(16).tobytes()
+    return _limbs(raw[:64] + _fq_bytes(-_fq_int(raw[i:i + 32]) % P_MOD for i in (64, 96)))
 
 
 def write_pk(E, pk, path):
@@ -568,7 +594,7 @@ def write_pk(E, pk, path):
     with open(path, "wb") as f:
         f.write(pk.k.to_bytes(4, "big") + len(pk.fixed_commitments).to_bytes(4, "big"))
         for pt in pk.fixed_commitments + pk.sigma_commitments:
-            f.write(_point_bytes(pt))
+            f.write(_fq_bytes(pt))
 
     def poly(b, rows):
         with open(path, "ab") as f:
@@ -606,8 +632,7 @@ def _point_check(raw):
         return "y is not less than the field modulus"
     if rx == 0 and ry == 0:
         return None
-    x, y = _point_from(raw)
-    return None if (y * y - x * x * x - 3) % P_MOD == 0 else "not on the curve"
+    return None if g1_on_curve(*_g1_from(raw)) else "not on the curve"
 
 
 def read_pk(E, cs, path, vk_digest=None, cosets="resident", format="RawBytesUnchecked"):
@@ -642,7 +667,7 @@ def read_pk(E, cs, path, vk_digest=None, cosets="resident", format="RawBytesUnch
             if why is not None:
                 what = "fixed commitment %d" % i if i < n_fixed else "sigma commitment %d" % (i - n_fixed)
                 raise ValueError("read_pk: %s: %s: %s" % (path, what, why))
-    pts = [_point_from(raw) for raw in raws]
+    pts = [_g1_from(raw) for raw in raws]
     n, ext = 1 << k, 1 << E.extended_k
     pk.cs, pk.k, pk.n = cs, k, n
     pk.blinding_factors = cs.blinding_factors(); pk.usable_rows = n - (pk.blinding_factors + 1)
@@ -713,6 +738,83 @@ def rotation_sets(queries_):
     return out
 
 
+def proof_evaluations(cs, n_sets, blinding_factors):
+    """(evals, openings) for a proof of `cs` with n_sets permutation sets. evals: the evaluations a proof carries, each as
+    (poly id, rotation), in transcript order: the advice queries, the fixed queries, the vanishing argument's random
+    polynomial, sigma, per permutation set z, z(omega X) and, but for the last set, z(omega^-(bf+1) X), per lookup z,
+    z(omega X), a', a'(omega^-1 X), s'. openings: create_proof's multi-open query order, which fixes SHPLONK's rotation sets,
+    as positions in evals; position len(evals) is h at x, the one query the transcript does not carry.
+    poly ids: ("advice", c), ("fixed", c), ("random",), ("sigma", c), ("perm", set), ("lk_z" | "lk_a" | "lk_s", lookup), ("h",)."""
+    last = -(blinding_factors + 1)
+    evals = [(("advice", c), r) for c, r in cs.advice_queries] + [(("fixed", c), r) for c, r in cs.fixed_queries]
+    evals += [(("random",), 0)] + [(("sigma", c), 0) for c in range(len(cs.permutation))]
+    for s in range(n_sets):
+        evals += [(("perm", s), 0), (("perm", s), 1)] + ([(("perm", s), last)] if s + 1 < n_sets else [])
+    for li in range(len(cs.lookups)):
+        evals += [(("lk_z", li), 0), (("lk_z", li), 1), (("lk_a", li), 0), (("lk_a", li), -1), (("lk_s", li), 0)]
+    at = {e: i for i, e in enumerate(evals)}
+    kinds = lambda *ks: [i for i, ((kind, *_), _) in enumerate(evals) if kind in ks]
+    openings = kinds("advice") + [at[(("perm", s), r)] for s in range(n_sets) for r in (0, 1)]
+    openings += [at[(("perm", s), last)] for s in reversed(range(n_sets - 1))]
+    openings += [at[e] for li in range(len(cs.lookups))
+                 for e in ((("lk_z", li), 0), (("lk_a", li), 0), (("lk_s", li), 0), (("lk_a", li), -1), (("lk_z", li), 1))]
+    return evals, openings + kinds("fixed", "sigma") + [len(evals), at[(("random",), 0)]]
+
+
+def _by_poly_id(advice, fixed, sigma, perm, lookup_z, lookup_a, lookup_s, random, h):
+    """{poly id of proof_evaluations: item}, the items of each kind given in column, set or lookup order"""
+    out = {("random",): random, ("h",): h}
+    for kind, items in (("advice", advice), ("fixed", fixed), ("sigma", sigma), ("perm", perm), ("lk_z", lookup_z), ("lk_a", lookup_a),
+                        ("lk_s", lookup_s)):
+        out.update(((kind, i), v) for i, v in enumerate(items))
+    return out
+
+
+def _intake(who, cs, n, usable, instances, advice_columns=None, E=None):
+    """Refuse instance and advice columns the circuit cannot take, as upstream does (`who` prefixes the message); advice is
+    checked when given. With an engine, the instance columns uploaded as create_proof lays them out: each column's values
+    at rows 0..len of an n-row buffer, zero below."""
+    if len(instances) != cs.num_instance:
+        raise ValueError("%s: %d instance columns given, the circuit has %d (upstream: Error::InvalidInstances)" % (who, len(instances), cs.num_instance))
+    if advice_columns is not None and len(advice_columns) != cs.num_advice:
+        raise ValueError("%s: %d advice columns given, the circuit has %d" % (who, len(advice_columns), cs.num_advice))
+    for col in instances:
+        if len(col) > usable:
+            raise ValueError("%s: an instance column has more than %d values (upstream: Error::InstanceTooLarge)" % (who, usable))
+    if E is None:
+        return None
+    values = []
+    for col in instances:
+        b = E.alloc(n); E.write_rows(b, 0, fr_mont_rows(col)); values.append(b)
+    return values
+
+
+def _permutation_columns(cs, fixed, advice, instance):
+    """the column behind each cs.permutation entry (kind, c): fixed[c], advice[c] or instance[c], whatever the containers hold"""
+    by_kind = {"fixed": fixed, "advice": advice, "instance": instance}
+    return [by_kind[kind][c] for kind, c in cs.permutation]
+
+
+def _compressed_lookup(E, pk, li, theta, advice_values, inst_values):
+    """lookup li's input and table expressions, each compressed with theta (a Horner sum over the tuple) into an n-row buffer"""
+    cs, n, zero4 = pk.cs, pk.n, fr_mont(0)
+    ci, ct = E.alloc(n), E.alloc(n)
+    for exprs, out in zip(cs.lookups[li], (ci, ct)):
+        E.graph_evaluate(cs.lookup_compress_program(exprs), pk.fixed_values, advice_values, inst_values, zero4, zero4, theta, zero4, out, n, 1)
+    return ci, ct
+
+
+def _stage_timer(E, timings):
+    """lap(name): with a timings dict, sync the engine and add the wall time since the previous lap (or since this call) to
+    timings[name]; without one, nothing"""
+    t_last = [time.perf_counter()]
+
+    def lap(name):
+        if timings is not None:
+            E.sync(); t = time.perf_counter(); timings[name] = timings.get(name, 0.0) + t - t_last[0]; t_last[0] = t
+    return lap
+
+
 # ---- create_proof -------------------------------------------------------------------------------------------------
 def evaluate_h_per_part(E, pk, advice_polys, inst_polys, perm_polys, lookups, beta, gamma, theta, y, lap):
     """Evaluator::evaluate_h one coset part at a time (a per-part key); returns the extended `values` (2^extended_k rows).
@@ -738,7 +840,7 @@ def evaluate_h_per_part(E, pk, advice_polys, inst_polys, perm_polys, lookups, be
     fixed_p, sigma_p, (l0, l_last, l_active) = take(len(pk.fixed_polys)), take(len(pk.sigma_polys)), take(3)
     advice_p, inst_p, z_p = take(len(advice_polys)), take(len(inst_polys)), take(len(perm_polys))
     lookup_p = [take(3) for _ in lookups]
-    cols = [{"fixed": fixed_p, "advice": advice_p, "instance": inst_p}[kind][c] for kind, c in cs.permutation]
+    cols = _permutation_columns(cs, fixed_p, advice_p, inst_p)
     gates = cs.gates_program() if cs.gates else None
     table_programs = [cs.lookup_value_program(li) for li in range(len(lookups))]
     part_values = E.alloc(n)
@@ -771,31 +873,18 @@ def create_proof(E, pk, instances, advice_columns, rng, transcript, timings=None
     instances: per instance column a list of ints; advice_columns: per advice column an (n, 4) Montgomery array whose
     rows >= usable_rows are overwritten with blinding; rng(count) -> (count, 4) Montgomery draws, consumed in
     upstream's order; transcript: EvmTranscriptWrite-like. Returns the proof bytes."""
-    import time
     cs, k, n = pk.cs, pk.k, pk.n
     bf, usable = pk.blinding_factors, pk.usable_rows
     ext_n, rot_scale = 1 << E.extended_k, 1 << (E.extended_k - k)
     G, GL = halo2.BASIS_G, halo2.BASIS_G_LAGRANGE
     w = omega_of(k)
-    t_last = [time.perf_counter()]
-
-    def lap(name):
-        if timings is not None:
-            E.sync(); t = time.perf_counter(); timings[name] = timings.get(name, 0.0) + t - t_last[0]; t_last[0] = t
+    lap = _stage_timer(E, timings)
 
     # 1. vk, instances
-    if len(instances) != cs.num_instance:
-        raise ValueError("create_proof: %d instance columns given, the circuit has %d (upstream: Error::InvalidInstances)" % (len(instances), cs.num_instance))
-    if len(advice_columns) != cs.num_advice:
-        raise ValueError("create_proof: %d advice columns given, the circuit has %d" % (len(advice_columns), cs.num_advice))
+    inst_values = _intake("create_proof", cs, n, usable, instances, advice_columns, E)
     for col in instances:
         for v in col:
             transcript.common_scalar(v)                      # KZG: instances enter the transcript, no commitments
-    inst_values = []
-    for col in instances:
-        if len(col) > usable:
-            raise ValueError("create_proof: an instance column has more than %d values (upstream: Error::InstanceTooLarge)" % usable)
-        b = E.alloc(n); E.write_rows(b, 0, fr_mont_rows(col)); inst_values.append(b)
     inst_polys = [E.clone(b) for b in inst_values]
     lagrange_to_coeff_many(E, inst_polys)
     lap("instances")
@@ -819,11 +908,9 @@ def create_proof(E, pk, instances, advice_columns, rng, transcript, timings=None
     # 3. lookups: compress, permute, commit
     class _L: pass
     lookups = []
-    for ins, tbs in cs.lookups:
+    for li in range(len(cs.lookups)):
         L = _L()
-        L.compressed_input, L.compressed_table = E.alloc(n), E.alloc(n)
-        E.graph_evaluate(cs.lookup_compress_program(ins), pk.fixed_values, advice_values, inst_values, zero4, zero4, theta, zero4, L.compressed_input, n, 1)
-        E.graph_evaluate(cs.lookup_compress_program(tbs), pk.fixed_values, advice_values, inst_values, zero4, zero4, theta, zero4, L.compressed_table, n, 1)
+        L.compressed_input, L.compressed_table = _compressed_lookup(E, pk, li, theta, advice_values, inst_values)
         L.permuted_input, L.permuted_table = E.alloc(n), E.alloc(n)
         E.permute_expression_pair(L.compressed_input, L.compressed_table, usable, L.permuted_input, L.permuted_table)
         E.write_rows(L.permuted_input, usable, rng(bf + 1))
@@ -840,7 +927,7 @@ def create_proof(E, pk, instances, advice_columns, rng, transcript, timings=None
     gamma = fr_mont(transcript.squeeze_challenge())
 
     # 4. permutation grand products, one per chunk of columns
-    col_values = [{"fixed": pk.fixed_values, "advice": advice_values, "instance": inst_values}[kind][c] for kind, c in cs.permutation]
+    col_values = _permutation_columns(cs, pk.fixed_values, advice_values, inst_values)
     chunk = cs.chunk_len()                                   # degree() >= 3, so >= 1
     perm_z, last_z = [], fr_mont(1)
     for lo in range(0, len(col_values), chunk):
@@ -902,7 +989,7 @@ def create_proof(E, pk, instances, advice_columns, rng, transcript, timings=None
             E.graph_evaluate(cs.gates_program(), fixed_cosets, advice_cosets, inst_cosets, beta, gamma, theta, y, values, ext_n, rot_scale)
         if perm_polys:
             z_cosets = coeff_to_extended_many(E, perm_polys)
-            cosets = [{"fixed": fixed_cosets, "advice": advice_cosets, "instance": inst_cosets}[kind][c] for kind, c in cs.permutation]
+            cosets = _permutation_columns(cs, fixed_cosets, advice_cosets, inst_cosets)
             ext_omega = fr_mont(pow(ROOT_OF_UNITY, 1 << (28 - E.extended_k), R_MOD))
             E.permutation_constraints(values, ext_n, rot_scale, -(bf + 1), chunk, z_cosets, cosets, sigma_cosets, l0, l_last, l_active, beta, gamma, y, ext_omega)
             del z_cosets, cosets
@@ -925,60 +1012,24 @@ def create_proof(E, pk, instances, advice_columns, rng, transcript, timings=None
     lap("vanishing_construct")
 
     x = transcript.squeeze_challenge()
-    xm = fr_mont(x)
     x_pow = lambda rot: x * pow(w, rot % n, R_MOD) % R_MOD
 
-    # 8. evaluations, in the order the verifier reads them. Every (polynomial, point) query is collected first and evaluated by
-    # ONE engine call (one kernel launch for the whole list), then the scalars enter the transcript in upstream's order.
-    polys, evals_q, todo = {}, [], []                        # poly id -> buffer; [(poly id, point, eval)] in multi-open order
-
-    def ask(pid, buf, rot):
-        polys[pid] = buf
-        todo.append((buf, x_pow(rot)))
-        return len(todo) - 1
-
-    adv_i = [ask(("advice", c), advice_polys[c], r) for c, r in cs.advice_queries]
-    fix_i = [ask(("fixed", c), pk.fixed_polys[c], r) for c, r in cs.fixed_queries]
+    # 8. evaluations: every (polynomial, point) query, h last, is evaluated by ONE engine call (one kernel launch for the whole
+    # list), then the scalars but h's enter the transcript in the order the verifier reads them.
     # vanishing::evaluate: h(X) = sum_i x^(n i) h_i(X), and the random polynomial at x
     h_poly = E.alloc(n)
     E.lincomb(h_pieces, fr_mont(pow(x, n, R_MOD)), h_poly, n)
-    rnd_i = ask(("random",), random_poly, 0)
-    sig_i = [ask(("sigma", c), pk.sigma_polys[c], 0) for c in range(len(pk.sigma_polys))]
-    perm_i = [(ask(("perm", s), p, 0), ask(("perm", s), p, 1), ask(("perm", s), p, -(bf + 1)) if s + 1 < len(perm_polys) else None)
-              for s, p in enumerate(perm_polys)]
-    look_i = [(ask(("lk_z", li), L.product_poly, 0), ask(("lk_z", li), L.product_poly, 1), ask(("lk_a", li), L.permuted_input_poly, 0),
-               ask(("lk_a", li), L.permuted_input_poly, -1), ask(("lk_s", li), L.permuted_table_poly, 0)) for li, L in enumerate(lookups)]
-    h_i = ask(("h",), h_poly, 0)
-    values = eval_polynomial_many(E, todo, n)
-    got = lambda i: None if i is None else (todo[i][1], values[i])
-    adv_e, fix_e, rnd_e, sig_e = [got(i) for i in adv_i], [got(i) for i in fix_i], got(rnd_i), [got(i) for i in sig_i]
-    perm_e = [tuple(got(i) for i in t) for t in perm_i]
-    look_e = [tuple(got(i) for i in t) for t in look_i]
-    for _, e in adv_e: transcript.write_scalar(e)
-    for _, e in fix_e: transcript.write_scalar(e)
-    transcript.write_scalar(rnd_e[1])
-    for _, e in sig_e: transcript.write_scalar(e)
-    for e0, e1, el in perm_e:
-        transcript.write_scalar(e0[1]); transcript.write_scalar(e1[1])
-        if el is not None:
-            transcript.write_scalar(el[1])
-    for t in look_e:
-        for _, e in t: transcript.write_scalar(e)
+    polys = _by_poly_id(advice_polys, pk.fixed_polys, pk.sigma_polys, perm_polys, [L.product_poly for L in lookups],
+                        [L.permuted_input_poly for L in lookups], [L.permuted_table_poly for L in lookups], random_poly, h_poly)
+    evals, openings = proof_evaluations(cs, len(perm_polys), bf)
+    asked = [(pid, x_pow(rot)) for pid, rot in evals + [(("h",), 0)]]
+    values = eval_polynomial_many(E, [(polys[pid], pt) for pid, pt in asked], n)
+    for e in values[:-1]:
+        transcript.write_scalar(e)
     lap("evaluations")
 
-    # 9. multi-open queries in create_proof's order: advice, permutation z, lookups, fixed, sigma, vanishing
-    for (c, r), (pt, e) in zip(cs.advice_queries, adv_e): evals_q.append((("advice", c), pt, e))
-    for s, (e0, e1, _) in enumerate(perm_e):
-        evals_q.append((("perm", s), e0[0], e0[1])); evals_q.append((("perm", s), e1[0], e1[1]))
-    for s in reversed(range(len(perm_e) - 1)):
-        el = perm_e[s][2]; evals_q.append((("perm", s), el[0], el[1]))
-    for li, (pe, pne, ie, iie, te) in enumerate(look_e):
-        evals_q += [(("lk_z", li), pe[0], pe[1]), (("lk_a", li), ie[0], ie[1]), (("lk_s", li), te[0], te[1]), (("lk_a", li), iie[0], iie[1]), (("lk_z", li), pne[0], pne[1])]
-    for (c, r), (pt, e) in zip(cs.fixed_queries, fix_e): evals_q.append((("fixed", c), pt, e))
-    for c, (pt, e) in enumerate(sig_e): evals_q.append((("sigma", c), pt, e))
-    h_eval = got(h_i)[1]
-    evals_q.append((("h",), x, h_eval)); evals_q.append((("random",), rnd_e[0], rnd_e[1]))
-
+    # 9. multi-open queries in create_proof's order
+    evals_q = [asked[i] + (values[i],) for i in openings]
     sets = [(fr_mont_rows(pts), [polys[p] for p in pids], np.stack([fr_mont_rows(row) for row in evs])) for pts, pids, evs in rotation_sets(evals_q)]
     y2 = fr_mont(transcript.squeeze_challenge())
     v = fr_mont(transcript.squeeze_challenge())
@@ -1015,15 +1066,7 @@ def check_witness(E, pk, instances, advice_columns, theta=None, max_rows=16):
     Instances are laid out as create_proof lays them out. A key whose sigma labels a cell outside the usable rows raises the
     engine's error naming the column and row."""
     cs, n, usable = pk.cs, pk.n, pk.usable_rows
-    if len(instances) != cs.num_instance:
-        raise ValueError("check_witness: %d instance columns given, the circuit has %d (upstream: Error::InvalidInstances)" % (len(instances), cs.num_instance))
-    if len(advice_columns) != cs.num_advice:
-        raise ValueError("check_witness: %d advice columns given, the circuit has %d" % (len(advice_columns), cs.num_advice))
-    inst_values = []
-    for col in instances:
-        if len(col) > usable:
-            raise ValueError("check_witness: an instance column has more than %d values (upstream: Error::InstanceTooLarge)" % usable)
-        b = E.alloc(n); E.write_rows(b, 0, fr_mont_rows(col)); inst_values.append(b)
+    inst_values = _intake("check_witness", cs, n, usable, instances, advice_columns, E)
     advice_values = [E.upload(col) for col in advice_columns]
     fixed = pk.fixed_values
     zero4 = fr_mont(0)
@@ -1038,15 +1081,13 @@ def check_witness(E, pk, instances, advice_columns, theta=None, max_rows=16):
             if total:
                 failures.append(WitnessFailure("gate", g, rows, total))
     theta = fr_mont(secrets.randbelow(R_MOD) if theta is None else theta)
-    for li, (ins, tbs) in enumerate(cs.lookups):
-        ci, ct = E.alloc(n), E.alloc(n)
-        E.graph_evaluate(cs.lookup_compress_program(ins), fixed, advice_values, inst_values, zero4, zero4, theta, zero4, ci, n, 1)
-        E.graph_evaluate(cs.lookup_compress_program(tbs), fixed, advice_values, inst_values, zero4, zero4, theta, zero4, ct, n, 1)
+    for li in range(len(cs.lookups)):
+        ci, ct = _compressed_lookup(E, pk, li, theta, advice_values, inst_values)
         rows, total = E.lookup_missing_rows(ci, ct, usable, max_rows)
         if total:
             failures.append(WitnessFailure("lookup", li, rows, total))
     if cs.permutation:
-        cols = [{"fixed": fixed, "advice": advice_values, "instance": inst_values}[kind][c] for kind, c in cs.permutation]
+        cols = _permutation_columns(cs, fixed, advice_values, inst_values)
         for c, (total, cells) in enumerate(E.copy_mismatches(cols, pk.sigma_values, usable, max_rows)):
             if total:
                 failures.append(WitnessFailure("copy", c, [r for r, _, _ in cells], total, [(c2, r2) for _, c2, r2 in cells]))
@@ -1082,12 +1123,7 @@ def check_pk(E, pk, max_rows=16, timings=None):
     commitment failures. The row comparisons go through one temporary of at most 2^extended_k rows (n rows for a lean key):
     recompute, subtract the stored buffer (vec_axpy with -1), report the nonzero rows. pk.vk_digest is not checked.
     timings: as create_proof's, a dict that gets the wall time of the stages commitments / polys / cosets / sigma."""
-    import time
-    t_last = [time.perf_counter()]
-
-    def lap(name):
-        if timings is not None:
-            E.sync(); t = time.perf_counter(); timings[name] = timings.get(name, 0.0) + t - t_last[0]; t_last[0] = t
+    lap = _stage_timer(E, timings)
     n, ext = pk.n, 1 << E.extended_k
     minus_one = fr_mont(R_MOD - 1)
     nf, m = len(pk.fixed_values), len(pk.sigma_values)
@@ -1155,11 +1191,6 @@ G2_GENERATOR = ((0x1800deef121f1e76426a00665e5c4479674322d4f75edadd46debd5cd992f
                 (0x12c85ea5db8c6deb4aab71808dcb408fe3d1e7690c43d37b4ce6cc0166fa7daa, 0x090689d0585ff075ec9e99ad690c3395bc4b313370b38ef355acdadcd122975b))
 
 
-def _g2_limbs(q):
-    """G2 affine ((x.c0, x.c1), (y.c0, y.c1)) ints -> uint64[16] Montgomery limbs in the params trailer's order"""
-    return np.frombuffer(b"".join((v * _FQ_MONT % P_MOD).to_bytes(32, "little") for c in q for v in c), dtype="<u8").astype(np.uint64)
-
-
 def check_params(E, be, vp=None, seed=None, timings=None):
     """Check that the points of the engine's params fit together: a list of ParamsFailure in the order of PARAMS_FAILURE_KINDS,
     [] for sound params. E: an engine bound to the params (E.params, E.k == params.k); be: anything with pairing_check_batch(ps,
@@ -1180,8 +1211,6 @@ def check_params(E, be, vp=None, seed=None, timings=None):
     Soundness: G1 has prime order r, so a wrong prefix passes one check with probability at most 1/r over the draws. The checks
     are random linear combinations: they cannot count failures, so each kind reports its first failure only.
     timings: a dict that gets the wall time of the stages points / powers / lagrange."""
-    import os
-    import time
     params = E.params
     if E.k != params.k:
         raise ValueError("check_params: the engine is for k = %d, the params for k = %d" % (E.k, params.k))
@@ -1200,11 +1229,7 @@ def check_params(E, be, vp=None, seed=None, timings=None):
     given = vp is not None
     vp = params.verifier_params() if vp is None else vp
     seed = os.urandom(32) if seed is None else seed
-    t_last = [time.perf_counter()]
-
-    def lap(name):
-        if timings is not None:
-            E.sync(); t = time.perf_counter(); timings[name] = timings.get(name, 0.0) + t - t_last[0]; t_last[0] = t
+    lap = _stage_timer(E, timings)
     drawn = [0]
 
     def draw(rows):
@@ -1217,7 +1242,7 @@ def check_params(E, be, vp=None, seed=None, timings=None):
     generator = _g1_limbs((1, 2))
     if not np.array_equal(g0, generator) or not np.array_equal(g0, vp.g):
         failures.append(ParamsFailure("g_generator", 0, "g[0] is %s, the G1 generator is (1, 2) and vp.g is %s"
-                                      % (_point_from(g0.tobytes()), _point_from(vp.g.tobytes()))))
+                                      % (_g1_from(g0.tobytes()), _g1_from(vp.g.tobytes()))))
     g2_ok = np.array_equal(vp.g2, _g2_limbs(G2_GENERATOR))
     if not g2_ok:
         failures.append(ParamsFailure("g2_generator", 0, "vp.g2 is not the G2 generator"))
@@ -1311,10 +1336,6 @@ class ProofFailure(namedtuple("ProofFailure", "kind detail")):
     opening, accumulator is reported. detail: a human-readable reason."""
 
 
-def _g1_limbs(pt):
-    return np.frombuffer(_point_bytes(pt), dtype="<u8").astype(np.uint64)
-
-
 def _multiexp(be, scalars, points):
     """sum_i scalars[i] points[i] on the backend, for ints and affine int points; the identity is (0, 0)"""
     return halo2.jacobian_to_affine_ints(be.best_multiexp(fr_mont_rows(scalars), np.stack([_g1_limbs(c) for c in points])))
@@ -1336,11 +1357,7 @@ def _opening_terms(vp, vk, instances, proof, transcript_read):
     n = 1 << k
     bf = cs.blinding_factors()
     usable = n - (bf + 1)
-    if len(instances) != cs.num_instance:
-        raise ValueError("verify_proof: %d instance columns given, the circuit has %d (upstream: Error::InvalidInstances)" % (len(instances), cs.num_instance))
-    for col in instances:
-        if len(col) > usable:
-            raise ValueError("verify_proof: an instance column has more than %d values (upstream: Error::InstanceTooLarge)" % usable)
+    _intake("verify_proof", cs, n, usable, instances)
     if len(vk.fixed_commitments) != cs.num_fixed or len(vk.sigma_commitments) != len(cs.permutation):
         raise ValueError("verify_proof: the verifying key has %d fixed and %d sigma commitments, the circuit %d and %d"
                          % (len(vk.fixed_commitments), len(vk.sigma_commitments), cs.num_fixed, len(cs.permutation)))
@@ -1370,15 +1387,8 @@ def _opening_terms(vp, vk, instances, proof, transcript_read):
         y = T.squeeze_challenge()
         h_c = [pt() for _ in range(cs.degree() - 1)]
         x = T.squeeze_challenge()
-        adv = {q: sc() for q in cs.advice_queries}
-        fix = {q: sc() for q in cs.fixed_queries}
-        random_eval = sc()
-        sigma_evals = [sc() for _ in cs.permutation]
-        perm_evals = []
-        for s in range(n_sets):
-            e0, e1 = sc(), sc()
-            perm_evals.append((e0, e1, sc() if s + 1 < n_sets else None))
-        look_evals = [tuple(sc() for _ in range(5)) for _ in cs.lookups]   # z, z_next, a', a'_inv, s'
+        evals, openings = proof_evaluations(cs, n_sets, bf)
+        got = dict(zip(evals, [sc() for _ in evals]))                  # (poly id, rotation) -> the proof's evaluation
         y2 = T.squeeze_challenge(); v = T.squeeze_challenge()
         h1 = pt()
         u = T.squeeze_challenge()
@@ -1398,12 +1408,13 @@ def _opening_terms(vp, vk, instances, proof, transcript_read):
     l0, l_last = L[0], L[usable]
     l_active = (1 - l_last - sum(L[i] for i in range(usable + 1, n))) % R
     inst = {(c, r): sum(val * L[i - r] for i, val in enumerate(instances[c])) % R for c, r in cs.instance_queries}
+    perm = lambda s, rot: got[(("perm", s), rot)]
+    look = lambda kind, li, rot: got[((kind, li), rot)]
 
     def ev(e):
         t = e[0]
         if t == "const": return e[1]
-        if t == "fixed": return fix[(e[1], e[2])]
-        if t == "advice": return adv[(e[1], e[2])]
+        if t in ("fixed", "advice"): return got[((t, e[1]), e[2])]
         if t == "instance": return inst[(e[1], e[2])]
         if t == "neg": return -ev(e[1]) % R
         if t == "sum": return (ev(e[1]) + ev(e[2])) % R
@@ -1414,20 +1425,22 @@ def _opening_terms(vp, vk, instances, proof, transcript_read):
     for g in cs.gates:
         acc = (acc * y + ev(g)) % R
     if n_sets:
-        col_eval = lambda kind, c: {"fixed": fix, "advice": adv, "instance": inst}[kind][(c, 0)]
-        acc = (acc * y + l0 * (1 - perm_evals[0][0])) % R
-        zl = perm_evals[-1][0]
+        cur = lambda kind, qs: {c: got[((kind, c), 0)] for c, r in qs if r == 0}
+        cols = _permutation_columns(cs, cur("fixed", cs.fixed_queries), cur("advice", cs.advice_queries),
+                                    {c: v for (c, r), v in inst.items() if r == 0})
+        acc = (acc * y + l0 * (1 - perm(0, 0))) % R
+        zl = perm(n_sets - 1, 0)
         acc = (acc * y + l_last * (zl * zl - zl)) % R
         for s in range(1, n_sets):
-            acc = (acc * y + l0 * (perm_evals[s][0] - perm_evals[s - 1][2])) % R
+            acc = (acc * y + l0 * (perm(s, 0) - perm(s - 1, -(bf + 1)))) % R
         for s in range(n_sets):
-            left, right = perm_evals[s][1], perm_evals[s][0]
+            left, right = perm(s, 1), perm(s, 0)
             for c in range(s * chunk, min((s + 1) * chunk, len(cs.permutation))):
-                kind, col = cs.permutation[c]
-                left = left * (col_eval(kind, col) + beta * sigma_evals[c] + gamma) % R
-                right = right * (col_eval(kind, col) + beta * x % R * pow(DELTA, c, R) + gamma) % R
+                left = left * (cols[c] + beta * got[(("sigma", c), 0)] + gamma) % R
+                right = right * (cols[c] + beta * x % R * pow(DELTA, c, R) + gamma) % R
             acc = (acc * y + l_active * (left - right)) % R
-    for (ins, tbs), (z, z_next, a_p, a_inv, s_p) in zip(cs.lookups, look_evals):
+    for li, (ins, tbs) in enumerate(cs.lookups):
+        z, z_next, a_p, a_inv, s_p = look("lk_z", li, 0), look("lk_z", li, 1), look("lk_a", li, 0), look("lk_a", li, -1), look("lk_s", li, 0)
         ci = ct = 0
         for e in ins: ci = (ci * theta + ev(e)) % R
         for e in tbs: ct = (ct * theta + ev(e)) % R
@@ -1440,25 +1453,13 @@ def _opening_terms(vp, vk, instances, proof, transcript_read):
 
     # ---- SHPLONK: the queries in create_proof's order, one linear combination of commitments per opening ------------
     xw = lambda r: x * pow(w, r % n, R) % R
-    q, commits = [], {}
-
-    def query(pid, terms, point, value):
-        commits[pid] = terms                                  # terms: [(scalar, point)] summing to the polynomial's commitment
-        q.append((pid, point, value))
-    for (c, r) in cs.advice_queries: query(("advice", c), [(1, advice_c[c])], xw(r), adv[(c, r)])
-    for s, (e0, e1, _) in enumerate(perm_evals):
-        query(("perm", s), [(1, perm_c[s])], x, e0); query(("perm", s), [(1, perm_c[s])], xw(1), e1)
-    for s in reversed(range(n_sets - 1)):
-        query(("perm", s), [(1, perm_c[s])], xw(-(bf + 1)), perm_evals[s][2])
-    for li, (z, z_next, a_p, a_inv, s_p) in enumerate(look_evals):
-        pin, ptab = permuted_c[li]
-        query(("lk_z", li), [(1, lookz_c[li])], x, z); query(("lk_a", li), [(1, pin)], x, a_p); query(("lk_s", li), [(1, ptab)], x, s_p)
-        query(("lk_a", li), [(1, pin)], xw(-1), a_inv); query(("lk_z", li), [(1, lookz_c[li])], xw(1), z_next)
-    for (c, r) in cs.fixed_queries: query(("fixed", c), [(1, vk.fixed_commitments[c])], xw(r), fix[(c, r)])
-    for c, e in enumerate(sigma_evals): query(("sigma", c), [(1, vk.sigma_commitments[c])], x, e)
-    query(("h",), [(pow(xn, i, R), hc) for i, hc in enumerate(h_c)], x, expected_h)       # h(X) = sum_i X^(n i) h_i(X)
-    query(("random",), [(1, random_c)], x, random_eval)
-    sets = rotation_sets(q)
+    # per polynomial, [(scalar, point)] summing to its commitment; h(X) = sum_i X^(n i) h_i(X)
+    one = lambda pts: [[(1, p)] for p in pts]
+    commits = _by_poly_id(one(advice_c), one(vk.fixed_commitments), one(vk.sigma_commitments), one(perm_c), one(lookz_c),
+                          one(a for a, _ in permuted_c), one(s for _, s in permuted_c), [(1, random_c)],
+                          [(pow(xn, i, R), hc) for i, hc in enumerate(h_c)])
+    asked = [(pid, xw(rot), got[(pid, rot)]) for pid, rot in evals] + [(("h",), x, expected_h)]
+    sets = rotation_sets([asked[i] for i in openings])
     super_pts = []
     for pts, _, _ in sets:
         for p in pts:
@@ -1490,23 +1491,13 @@ def _opening_terms(vp, vk, instances, proof, transcript_read):
     zt = 1
     for p in super_pts: zt = zt * (u - p) % R
     z0_inv = inv(z0)
-    g = _point_from(vp.g.tobytes())
+    g = _g1_from(vp.g.tobytes())
     terms[g] = (terms.get(g, 0) - const) % R
     terms[h1] = (terms.get(h1, 0) - zt) % R
     bases = [c for c in terms]
     scalars = [terms[c] * z0_inv % R for c in bases]
     bases.append(h2); scalars.append(u)
     return scalars, bases, h2
-
-
-def _neg_g2(q):
-    """-Q for a G2 affine point as uint64[16] Montgomery limbs (x.c0, x.c1, y.c0, y.c1): both y coordinates negated mod p"""
-    out = np.array(q, dtype=np.uint64).reshape(4, 4).copy()
-    for c in (2, 3):
-        v = int(out[c, 0]) | int(out[c, 1]) << 64 | int(out[c, 2]) << 128 | int(out[c, 3]) << 192
-        v = (P_MOD - v) % P_MOD
-        out[c] = [(v >> (64 * j)) & 0xFFFFFFFFFFFFFFFF for j in range(4)]
-    return out.reshape(16)
 
 
 # ---- the KZG accumulator of an aggregation proof ----------------------------------------------------------------------
@@ -1523,7 +1514,7 @@ ACCUMULATOR_LIMBS, ACCUMULATOR_LIMB_BITS = 3, 88
 # (column, row) of the 12 accumulator limbs among the instances, as snark-verifier's accumulator_indices: Spectre's
 # aggregation circuits put them first in their one instance column
 AGGREGATION_ACCUMULATOR_INDICES = [(0, i) for i in range(4 * ACCUMULATOR_LIMBS)]
-_M256 = (1 << 256) - 1
+_M256 = MONT_RADIX - 1                                  # an EVM word wraps mod 2^256
 
 
 def accumulator_to_limbs(acc):
@@ -1548,9 +1539,8 @@ def accumulator_from_limbs(words):
             v = (v + (limb << (ACCUMULATOR_LIMB_BITS * i))) & _M256
         coords.append(v)
     pts = [(coords[0], coords[1]), (coords[2], coords[3])]
-    for x, y in pts:
-        if x >= P_MOD or y >= P_MOD or (y * y - x * x * x - 3) % P_MOD:
-            return None
+    if not all(g1_on_curve(x, y) for x, y in pts):
+        return None
     return KzgAccumulator(*pts)
 
 

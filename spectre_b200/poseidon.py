@@ -25,8 +25,7 @@ Two layers, with different pinning:
   snark-verifier's own transcript (INTEGRATION.md); this module exists so that the in-repo drivers can run the same protocol
   over either transcript, and is self-consistent with tests/plonk_verifier.py.
 """
-R_MOD = 0x30644e72e131a029b85045b68181585d2833e84879b9709143e1f593f0000001
-P_MOD = 0x30644e72e131a029b85045b68181585d97816a916871ca8d3c208c16d87cfd47
+from .halo2 import P_MOD, R_MOD, g1_on_curve
 
 
 def _grain_bits(field_bits, t, r_f, r_p):
@@ -150,7 +149,7 @@ def decompress_g1(b):
     if x >= P_MOD:
         raise ValueError("non-canonical x coordinate in proof")
     y = pow((x * x * x + 3) % P_MOD, (P_MOD + 1) // 4, P_MOD)          # p = 3 mod 4
-    if (y * y - x * x * x - 3) % P_MOD:
+    if not g1_on_curve(x, y):
         raise ValueError("proof point is not on the curve")
     return (x, y if (y & 1) == odd else P_MOD - y)
 

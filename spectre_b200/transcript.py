@@ -12,8 +12,7 @@ verifier contracts, which replay it in Yul (contracts/snark-verifiers/sync_step_
 The transcript is the caller's side of the C ABI (it orders the calls and owns the challenges); nothing here is on
 the GPU hot path. hashlib has SHA-3 but not the original Keccak padding, so Keccak-f[1600] is spelled out below.
 """
-R_MOD = 0x30644e72e131a029b85045b68181585d2833e84879b9709143e1f593f0000001
-P_MOD = 0x30644e72e131a029b85045b68181585d97816a916871ca8d3c208c16d87cfd47
+from .halo2 import R_MOD, g1_on_curve
 
 _RC = [0x0000000000000001, 0x0000000000008082, 0x800000000000808A, 0x8000000080008000, 0x000000000000808B, 0x0000000080000001,
        0x8000000080008081, 0x8000000000008009, 0x000000000000008A, 0x0000000000000088, 0x0000000080008009, 0x000000008000000A,
@@ -108,7 +107,7 @@ class EvmTranscriptRead(EvmTranscriptWrite):
 
     def read_ec_point(self):
         x = int.from_bytes(self.stream[self.pos:self.pos + 32], "big"); y = int.from_bytes(self.stream[self.pos + 32:self.pos + 64], "big"); self.pos += 64
-        if x >= P_MOD or y >= P_MOD or (y * y - x * x * x - 3) % P_MOD:
+        if not g1_on_curve(x, y):
             raise ValueError("proof point is not on the curve")
         self.common_ec_point((x, y))
         return (x, y)
