@@ -156,8 +156,8 @@ int spb_srs_precompute(spb_ctx* ctx, spb_srs* srs);
 /* number of G1 additions (mixed + full) the last MSM executed on the device(s) */
 uint64_t spb_last_msm_adds(spb_ctx* ctx);
 /* device milliseconds of the last MSM's stages on the context's first device, from CUDA events on the stream the
- * kernels ran on: [0] digit histogram, [1] bucket-offset scan, [2] scatter, [3] bucket accumulation (the dominant
- * kernel), [4] chain stitch, [5] bucket groups (running sums over 8 buckets per thread), [6] row/column tree sums of the
+ * kernels ran on: [0] signed digits into an unsorted entry list, [1] the entry count's trip to the host and the radix sort
+ * of the entries by bucket, [2] bucket offsets of the sorted list, [3] bucket accumulation (the dominant kernel), [4] chain stitch, [5] bucket groups (running sums over 8 buckets per thread), [6] row/column tree sums of the
  * group sums + weighted partial sums. */
 void spb_last_msm_stage_ms(spb_ctx* ctx, float out[7]);
 /* window width c and window count the library uses for an n-pair MSM (tables: with spb_srs_precompute) */

@@ -33,7 +33,7 @@ struct NttTables {
 // batch cycle over the lanes so the latency-bound tail of one overlaps the sort and accumulation of the next (msm.cu).
 struct MsmLane {
   cudaStream_t stream = nullptr;
-  cudaEvent_t ev[9] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+  cudaEvent_t ev[10] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};  // 0-7 stage bounds, 8 start, 9 entry count on the host
   void* pinned = nullptr;
   bool ready = false;
 };
@@ -71,7 +71,7 @@ struct spb_ctx {
   float last_kernel_ms = 0.f;
   uint64_t last_msm_adds = 0;  // G1 additions of the last MSM call / batch
   bool shplonk_slots_busy = false;  // the context's SHPLONK workspace slots are held by an open spb_shplonk handle
-  float msm_stage_ms[7] = {0, 0, 0, 0, 0, 0, 0};  // count, scan, scatter, accumulate, stitch, segment, window (device 0)
+  float msm_stage_ms[7] = {0, 0, 0, 0, 0, 0, 0};  // digits, sort, offsets, accumulate, stitch, groups, rowcol + weighted (device 0)
 };
 
 // EvaluationDomain (capi.cu builds it; quotient.cu reads its sizes)

@@ -2,7 +2,7 @@
 #define SPB_MSM_KERNELS 1
 #include "common.cuh"
 #include "msm.cuh"
-#include <cub/device/device_scan.cuh>
+#include <cub/device/device_radix_sort.cuh>
 #include <string.h>
 
 using namespace spb;
@@ -33,7 +33,7 @@ static int get_lane(spb_ctx* ctx, int dev_index, int lane_index, Lane** out) {
   Lane& l = ctx->dev[dev_index].lanes[lane_index];
   if (!l.ready) {
     SPB_CUDA(ctx, cudaStreamCreateWithFlags(&l.stream, cudaStreamNonBlocking));
-    for (int i = 0; i < 9; i++) SPB_CUDA(ctx, cudaEventCreate(&l.ev[i]));
+    for (int i = 0; i < 10; i++) SPB_CUDA(ctx, cudaEventCreate(&l.ev[i]));
     SPB_CUDA(ctx, cudaMallocHost(&l.pinned, kLanePinnedBytes));
     l.ready = true;
   }
@@ -47,7 +47,7 @@ void msm_release_ctx(spb_ctx* ctx) {
     for (auto& l : d.lanes) {
       if (!l.ready) continue;
       cudaStreamSynchronize(l.stream);
-      for (int i = 0; i < 9; i++) cudaEventDestroy(l.ev[i]);
+      for (int i = 0; i < 10; i++) cudaEventDestroy(l.ev[i]);
       cudaFreeHost(l.pinned);
       cudaStreamDestroy(l.stream);
       l = Lane();
@@ -76,17 +76,52 @@ static uint32_t choose_chunk(const DeviceState& d, uint64_t est_entries) {
   return L;
 }
 
-// Enqueue one MSM on lane `ln` of device `d` (no host synchronisation). The BW window sums land in the lane's
-// pinned area, followed by the 32-bit number of sorted entries.
-static int msm_enqueue(spb_ctx* ctx, DeviceState& d, int lane, Lane& ln, const Fr* d_scalars, const G1Affine* d_bases, uint64_t n, MsmGeom g) {
-  const uint64_t nb = (uint64_t)g.BW * g.B;
+// Workspace of one MSM on a lane: the slots are named per lane, so both halves of msm_enqueue_* find the same buffers.
+struct MsmWork {
+  uint32_t* total;          // entry count M, counted by the digit kernel
+  MsmEntry* ent[2];         // unsorted entries | the radix sort's other buffer
+  void* sort_tmp; size_t sort_bytes;
+};
+static int msm_work(spb_ctx* ctx, DeviceState& d, int lane, Lane& ln, uint64_t n, MsmGeom g, MsmWork& w) {
   const uint64_t cap = n * g.W;                 // upper bound on entries
+  if (cap >= 0x7fffffffull) return set_error(ctx, SPB_ERR_ARG, "msm: %llu entries exceed the 31-bit sort index", (unsigned long long)cap);
+  w.total = (uint32_t*)lane_slot(ctx, d, lane, "msm_total", 16);
+  w.ent[0] = (MsmEntry*)lane_slot(ctx, d, lane, "msm_entries", (cap + 1) * sizeof(MsmEntry));
+  w.ent[1] = (MsmEntry*)lane_slot(ctx, d, lane, "msm_entries_alt", (cap + 1) * sizeof(MsmEntry));
+  // temporary storage for the longest list this MSM can have; a shorter sort uses a prefix of it
+  cub::DoubleBuffer<uint64_t> keys((uint64_t*)w.ent[0], (uint64_t*)w.ent[1]);
+  w.sort_bytes = 0;
+  SPB_CUDA(ctx, cub::DeviceRadixSort::SortKeys(nullptr, w.sort_bytes, keys, (int)cap, 0, msm_key_bits(g), ln.stream));
+  w.sort_tmp = lane_slot(ctx, d, lane, "msm_sort_tmp", w.sort_bytes ? w.sort_bytes : 16);
+  if (!w.total || !w.ent[0] || !w.ent[1] || !w.sort_tmp) return SPB_ERR_OOM;
+  return 0;
+}
+
+// First half of one MSM on lane `ln` of device `d`: the digit kernel writes the unsorted entries and counts them; the count
+// is copied to the lane's pinned area (after the window partials) and ln.ev[9] marks its arrival.
+static int msm_enqueue_digits(spb_ctx* ctx, DeviceState& d, int lane, Lane& ln, const Fr* d_scalars, uint64_t n, MsmGeom g) {
+  MsmWork w; SPB_TRY(msm_work(ctx, d, lane, ln, n, g, w));
+  const uint32_t per = msm_tail_partials(msm_tail_shape(g.c));
+  if ((size_t)g.BW * per * sizeof(G1Xyzz) + 16 > kLanePinnedBytes) return set_error(ctx, SPB_ERR_STATE, "msm: %u window partials exceed the pinned staging area", g.BW * per);
+  cudaStream_t st = ln.stream;
+  SPB_CUDA(ctx, cudaMemsetAsync(w.total, 0, 4, st));
+  cudaEventRecord(ln.ev[0], st);
+  SPB_TRY(launch(ctx, st, nblk(n, kDigitsThreads), kDigitsThreads, 0, msm_digits_kernel, n, d_scalars, g, w.total, w.ent[0]));
+  cudaEventRecord(ln.ev[1], st);
+  SPB_CUDA(ctx, cudaMemcpyAsync((char*)ln.pinned + (size_t)g.BW * per * sizeof(G1Xyzz), w.total, 4, cudaMemcpyDeviceToHost, st));
+  SPB_CUDA(ctx, cudaEventRecord(ln.ev[9], st));
+  return 0;
+}
+
+// Second half: waits for the entry count M on the host (the device keeps running whatever the other lanes have queued), then
+// enqueues the sort of exactly M entries and the rest of the MSM. The BW window sums land in the lane's pinned area.
+static int msm_enqueue_rest(spb_ctx* ctx, DeviceState& d, int lane, Lane& ln, const G1Affine* d_bases, uint64_t n, MsmGeom g) {
+  MsmWork w; SPB_TRY(msm_work(ctx, d, lane, ln, n, g, w));
+  const uint64_t nb = (uint64_t)g.BW * g.B;
+  const uint64_t cap = n * g.W;
   const uint32_t Lmin = g.L == kLongChunk ? kShortChunk : g.L;   // the kernels may fall back to the short chunk (msm_effective_chunk)
   const uint64_t Tmax = (cap + Lmin - 1) / Lmin;  // upper bound on chunks
-  if (cap >= 0x7fffffffull) return set_error(ctx, SPB_ERR_ARG, "msm: %llu entries exceed the 31-bit sort index", (unsigned long long)cap);
-  uint32_t* counts = (uint32_t*)lane_slot(ctx, d, lane, "msm_counts", (nb + 1) * 4);
   uint32_t* offsets = (uint32_t*)lane_slot(ctx, d, lane, "msm_offsets", (nb + 1) * 4);
-  MsmEntry* ent = (MsmEntry*)lane_slot(ctx, d, lane, "msm_entries", (cap + 1) * sizeof(MsmEntry));
   G1Xyzz* buckets = (G1Xyzz*)lane_slot(ctx, d, lane, "msm_buckets", nb * sizeof(G1Xyzz));
   uint32_t* head_key = (uint32_t*)lane_slot(ctx, d, lane, "msm_head_key", (Tmax + 1) * 4);
   uint32_t* tail_key = (uint32_t*)lane_slot(ctx, d, lane, "msm_tail_key", (Tmax + 1) * 4);
@@ -103,31 +138,24 @@ static int msm_enqueue(spb_ctx* ctx, DeviceState& d, int lane, Lane& ln, const F
   G1Xyzz* grp = (G1Xyzz*)lane_slot(ctx, d, lane, "msm_groups", 2 * ngroups * sizeof(G1Xyzz));   // S1 | W1
   G1Xyzz* seg_out = (G1Xyzz*)lane_slot(ctx, d, lane, "msm_rowcol", (uint64_t)g.BW * (2 * R + C) * sizeof(G1Xyzz));   // rows | columns | W rows
   G1Xyzz* win_out = (G1Xyzz*)lane_slot(ctx, d, lane, "msm_partials", (uint64_t)g.BW * per * sizeof(G1Xyzz));
-  size_t scan_bytes = 0;
-  cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, counts, offsets, (int)(nb + 1), ln.stream);
-  void* scan_tmp = lane_slot(ctx, d, lane, "msm_scan_tmp", scan_bytes ? scan_bytes : 16);
-  if (!counts || !offsets || !ent || !buckets || !head_key || !tail_key || !head || !tail || !giant || !huge || !huge_part || !grp || !seg_out || !win_out || !scan_tmp)
+  if (!offsets || !buckets || !head_key || !tail_key || !head || !tail || !giant || !huge || !huge_part || !grp || !seg_out || !win_out)
     return SPB_ERR_OOM;
-  if ((size_t)g.BW * per * sizeof(G1Xyzz) + 16 > kLanePinnedBytes) return set_error(ctx, SPB_ERR_STATE, "msm: %u window partials exceed the pinned staging area", g.BW * per);
 
+  SPB_CUDA(ctx, cudaEventSynchronize(ln.ev[9]));
+  uint32_t M; memcpy(&M, (const char*)ln.pinned + (size_t)g.BW * per * sizeof(G1Xyzz), 4);
   cudaStream_t st = ln.stream;
   // the bucket array is NOT cleared: every non-empty bucket is written exactly once (accumulate / stitch / giant paths) and
-  // the reduction reads a bucket only where the sort's offsets say it has entries
+  // the reduction reads a bucket only where the offsets say it has entries
   SPB_CUDA(ctx, cudaMemsetAsync(giant, 0, 4, st));
   SPB_CUDA(ctx, cudaMemsetAsync(huge, 0, 4, st));
-  const unsigned tb = 256;
-  SPB_CUDA(ctx, cudaMemsetAsync(counts, 0, (nb + 1) * 4, st));
-  cudaEventRecord(ln.ev[0], st);
-  SPB_TRY(launch(ctx, st, nblk(n, tb), tb, 0, msm_count_kernel, n, d_scalars, g, counts));
-  cudaEventRecord(ln.ev[1], st);
-  SPB_CUDA(ctx, cub::DeviceScan::ExclusiveSum(scan_tmp, scan_bytes, counts, offsets, (int)(nb + 1), st));
-  // cursor := offsets (the counters are dead after the scan; reuse their storage)
-  SPB_CUDA(ctx, cudaMemcpyAsync(counts, offsets, (nb + 1) * 4, cudaMemcpyDeviceToDevice, st));
+  // Sorting M entries rather than the n * W upper bound keeps a sparse (witness) column as cheap as its entries. A pass
+  // moves whole 8-byte entries but looks only at key bits: the value in the upper half rides along.
+  cub::DoubleBuffer<uint64_t> keys((uint64_t*)w.ent[0], (uint64_t*)w.ent[1]);
+  SPB_CUDA(ctx, cub::DeviceRadixSort::SortKeys(w.sort_tmp, w.sort_bytes, keys, (int)M, 0, msm_key_bits(g), st));
+  const MsmEntry* ent = (const MsmEntry*)keys.Current();
+  const uint32_t* total = w.total;
   cudaEventRecord(ln.ev[2], st);
-  // (Two alternatives to this one-pass counting sort were built and measured slower at every size -- a second scatter pass with
-  // L2-resident write windows, and a bin-local sort ranking in shared memory.)
-  SPB_TRY(launch(ctx, st, nblk(n, tb), tb, 0, msm_scatter_kernel, n, d_scalars, g, counts, ent));
-  const uint32_t* total = offsets + nb;  // number of entries M, resident on the device
+  SPB_TRY(launch(ctx, st, nblk(nb + 1, 256), 256, 0, msm_offsets_kernel, total, nb, ent, offsets));
   cudaEventRecord(ln.ev[3], st);
   SPB_TRY(launch(ctx, st, nblk(Tmax, 128), 128, 0, msm_accumulate_kernel, total, g, ent, d_bases, buckets, head_key, head, tail_key, tail));
   cudaEventRecord(ln.ev[4], st);
@@ -143,7 +171,6 @@ static int msm_enqueue(spb_ctx* ctx, DeviceState& d, int lane, Lane& ln, const F
   SPB_TRY(launch(ctx, st, g.BW * (2 * tl.nbr + tl.nbc), 128, 0, msm_weighted_kernel, tl, rows, cols, wrows, win_out));
   cudaEventRecord(ln.ev[7], st);
   SPB_CUDA(ctx, cudaMemcpyAsync(ln.pinned, win_out, (size_t)g.BW * per * sizeof(G1Xyzz), cudaMemcpyDeviceToHost, st));
-  SPB_CUDA(ctx, cudaMemcpyAsync((char*)ln.pinned + (size_t)g.BW * per * sizeof(G1Xyzz), total, 4, cudaMemcpyDeviceToHost, st));
   return 0;
 }
 
@@ -174,7 +201,8 @@ struct MsmPart {
   MsmGeom g;
 };
 
-// One job = one MSM = one part per device, all on lane `lane`. enqueue -> (later) collect.
+// One job = one MSM = one part per device, all on lane `lane`. enqueue -> (later) collect. The enqueue returns once every
+// part's entry count has reached the host and the rest of the part is queued.
 static int job_enqueue(spb_ctx* ctx, int lane, std::vector<MsmPart>& parts) {
   for (auto& p : parts) {
     if (!p.n) continue;
@@ -197,7 +225,15 @@ static int job_enqueue(spb_ctx* ctx, int lane, std::vector<MsmPart>& parts) {
       else SPB_CUDA(ctx, cudaMemcpyPeerAsync(buf, d.device, p.d_scalars, p.peer_src_device, p.n * sizeof(Fr), ln->stream));
       ds = buf;
     }
-    SPB_TRY(msm_enqueue(ctx, d, lane, *ln, ds, p.d_bases, p.n, p.g));
+    SPB_TRY(msm_enqueue_digits(ctx, d, lane, *ln, ds, p.n, p.g));
+  }
+  // every part's digit kernel is queued before the first wait for an entry count
+  for (auto& p : parts) {
+    if (!p.n) continue;
+    DeviceState& d = ctx->dev[p.dev_index];
+    SPB_CUDA(ctx, cudaSetDevice(d.device));
+    Lane* ln; SPB_TRY(get_lane(ctx, p.dev_index, lane, &ln));
+    SPB_TRY(msm_enqueue_rest(ctx, d, lane, *ln, p.d_bases, p.n, p.g));
   }
   return 0;
 }
@@ -625,12 +661,13 @@ static int msm_batch_common(spb_ctx* ctx, const spb_srs* srs, int basis, const s
   if (!ctx || !srs || !out || (count && !scalars)) return SPB_ERR_ARG;
   std::lock_guard<std::mutex> lk(ctx->mu);
   ctx->last_msm_adds = 0;
-  // every lane holds a workspace sized for these MSMs (sorted entries, chunk pieces, buckets); lanes beyond the first are
-  // used only while their workspaces together stay within a tenth of the device's memory (H100, 80 GB: three lanes for a
-  // K = 23 SRS with tables, one for K = 24 without), so a large proof keeps its memory for its polynomials
+  // every lane holds a workspace sized for these MSMs (the entries and the sort's second buffer, chunk pieces, buckets); lanes
+  // beyond the first are used only while their workspaces together stay within a tenth of the device's memory (H100, 80 GB:
+  // three lanes for a K = 23 SRS with tables, 2.7 GB each; one for K = 24 without, 6.2 GB), so a large proof keeps its memory
+  // for its polynomials. (The sort's temporary storage, a few MB, is left out.)
   const MsmGeom lg = srs->table_c ? msm_make_geometry(srs->table_c, true, 0) : msm_choose_geometry(n ? n : 1);
   const uint64_t ents = (uint64_t)n * lg.W;
-  const uint64_t lane_bytes = ents * sizeof(MsmEntry) + 2 * (ents / kShortChunk + 1) * (sizeof(G1Xyzz) + 4) + (uint64_t)lg.BW * lg.B * sizeof(G1Xyzz);
+  const uint64_t lane_bytes = 2 * ents * sizeof(MsmEntry) + 2 * (ents / kShortChunk + 1) * (sizeof(G1Xyzz) + 4) + (uint64_t)lg.BW * lg.B * sizeof(G1Xyzz);
   const uint64_t fit = ctx->dev[0].total_mem / 10 / (lane_bytes ? lane_bytes : 1);
   const size_t NL = std::max<size_t>(1, std::min<size_t>((size_t)kMaxMsmLanes, (size_t)fit));
   std::vector<MsmPart> jobs[kMaxMsmLanes];

@@ -1,5 +1,5 @@
 // BN254 G1 multi-scalar multiplication for sm_90a: signed-digit windowed Pippenger with a
-// counting sort and a load-balanced segmented bucket accumulation.
+// radix sort of the digits and a load-balanced segmented bucket accumulation.
 //
 // Replaces halo2_proofs::arithmetic::best_multiexp / multiexp_serial ([UPSTREAM] halo2_proofs/src/arithmetic.rs;
 // reached from every ParamsKZG::commit / commit_lagrange inside create_proof and keygen, reference call sites
@@ -9,11 +9,12 @@
 //
 // Pipeline (one MSM of n pairs, window width c, W = ceil(255/c) windows, B = 2^(c-1) buckets per bucket set; a basis
 // with precomputed 2^(c*w) multiples folds all windows into ONE bucket set, otherwise there are W sets):
-//   1. digits   : Montgomery -> canonical scalar (one product), signed c-bit digits d_w in (-B, B], histogram
-//                 of (w, |d_w|) with global atomics; zero digits are dropped here.
-//   2. scan     : exclusive prefix sum of the W*B counters (bucket offsets).
-//   3. scatter  : each non-zero digit writes (key = w*B + |d|-1, value = point index | sign << 31) at
-//                 atomicAdd(cursor[key]) -- a counting sort; order inside a bucket is irrelevant.
+//   1. digits   : Montgomery -> canonical scalar (one product), signed c-bit digits d_w in (-B, B]; every non-zero digit
+//                 becomes an entry (key = w*B + |d|-1, value = point index | sign << 31) in an unsorted list, compacted
+//                 with one atomic per block. Zero digits are dropped here; the entry count M goes to the host.
+//   2. sort     : LSD radix sort of the M entries by key (CUB onesweep over the key's bit length only); order inside a
+//                 bucket is irrelevant.
+//   3. offsets  : offsets[k] = first entry of bucket k (every bucket, empty ones included; offsets[BW*B] = M).
 //   4. accumulate: the sorted entry list is cut into fixed chunks of L entries, ONE THREAD PER CHUNK, so every
 //                 thread performs the same number of mixed XYZZ additions whatever the digit distribution
 //                 (witness columns put hundreds of thousands of points into one bucket). A run of equal keys
@@ -98,7 +99,58 @@ struct DigitIter {
   }
 };
 
-// ---- step 1: histogram ---------------------------------------------------------------------------------
+// ---- step 1: digits -> unsorted entries -----------------------------------------------------------------------
+SPB_HD MsmEntry msm_make_entry(uint64_t tid, uint32_t w, int32_t d, const MsmGeom& g) {
+  const uint32_t mag = d < 0 ? (uint32_t)(-d) : (uint32_t)d;
+  MsmEntry e;
+  e.key = (g.precomp ? 0u : w * g.B) + mag - 1;
+  e.val = ((uint32_t)tid + (g.precomp ? w * g.tab_stride : 0u)) | (d < 0 ? 0x80000000u : 0u);
+  return e;
+}
+// number of non-zero signed digits of a canonical scalar
+SPB_HD uint32_t msm_digit_count(const Fr& s, const MsmGeom& g) {
+  DigitIter it; it.init(s, g.c);
+  uint32_t k = 0;
+  for (uint32_t w = 0; w < g.W; w++) k += it.next() != 0;
+  return k;
+}
+// Serial form of msm_digits_kernel: scalar `tid` reserves its entries with one counter increment and writes them in window
+// order. The kernel reserves one range per block instead and writes each window of a warp contiguously; the list is sorted
+// next, so only the multiset of entries matters.
+SPB_HD void msm_digits_thread(uint64_t tid, uint64_t n, const Fr* scalars, MsmGeom g, uint32_t* total, MsmEntry* ent) {
+  if (tid >= n) return;
+  Fr s = fp_from_mont(scalars[tid]);
+  if (fp_is_zero(s)) return;
+  uint32_t pos = *total;
+  *total = pos + msm_digit_count(s, g);
+  DigitIter it; it.init(s, g.c);
+  for (uint32_t w = 0; w < g.W; w++) {
+    int32_t d = it.next();
+    if (d != 0) ent[pos++] = msm_make_entry(tid, w, d, g);
+  }
+}
+
+// ---- step 2: the radix sort looks at the bits of the largest bucket key BW*B - 1 only ------------------------------
+inline int msm_key_bits(const MsmGeom& g) {
+  int bits = 0;
+  for (uint64_t k = (uint64_t)g.BW * g.B - 1; k; k >>= 1) bits++;
+  return bits;
+}
+
+// ---- step 3: bucket offsets of the sorted list ------------------------------------------------------------------
+// offsets[k] = number of entries with key < k, for every k in [0, nb] (so offsets[nb] = M): a lower-bound search per bucket,
+// which costs the same for empty buckets, sparse lists and M = 0.
+SPB_HD void msm_offsets_thread(uint64_t k, uint64_t nb, uint64_t M, const MsmEntry* sorted, uint32_t* offsets) {
+  if (k > nb) return;
+  uint64_t lo = 0, hi = M;
+  while (lo < hi) {
+    const uint64_t mid = (lo + hi) >> 1;
+    if (sorted[mid].key < k) lo = mid + 1; else hi = mid;
+  }
+  offsets[k] = (uint32_t)lo;
+}
+
+// ---- serial reference of steps 1-3: a counting sort (histogram, exclusive scan, scatter at a cursor) ----------------
 SPB_HD void msm_count_thread(uint64_t tid, uint64_t n, const Fr* scalars, MsmGeom g, uint32_t* counts) {
   if (tid >= n) return;
   Fr s = fp_from_mont(scalars[tid]);
@@ -112,7 +164,6 @@ SPB_HD void msm_count_thread(uint64_t tid, uint64_t n, const Fr* scalars, MsmGeo
   }
 }
 
-// ---- step 3: scatter -----------------------------------------------------------------------------------
 SPB_HD void msm_scatter_thread(uint64_t tid, uint64_t n, const Fr* scalars, MsmGeom g, uint32_t* cursor, MsmEntry* ent) {
   if (tid >= n) return;
   Fr s = fp_from_mont(scalars[tid]);
@@ -218,7 +269,7 @@ SPB_HD void msm_stitch_thread(uint64_t tid, uint64_t T, uint32_t cap, const uint
 // Two levels, both free of scalar multiples and of long running sums:
 //  (a) groups: thread t takes the m = 2^m_log consecutive buckets b = t*m + j and forms, with one running sum from the top,
 //      S1_t = sum_j B_{t*m+j} and W1_t = sum_j j * B_{t*m+j} (2m - 1 additions, no synchronisation, every thread busy).
-//      Empty buckets are recognised from the bucket offsets of the counting sort, so the bucket array is never cleared
+//      Empty buckets are recognised from the bucket offsets of the sort (step 3), so the bucket array is never cleared
 //      and never read where nothing was written. Then S_w = sum_t W1_t + sum_t S1_t + m * sum_t t * S1_t.
 //  (b) the T = B / m group sums S1 are viewed as an R x C matrix (t = r*C + c):
 //      sum_t t*S1_t = C * sum_r r*Row_r + sum_c c*Col_c,   Row_r = sum_c S1[r][c],  Col_c = sum_r S1[r][c]
@@ -242,7 +293,7 @@ inline MsmTail msm_tail_shape(uint32_t c) {
 // Col_{128j+i}, V[j] = sum_i WRow_{128j+i} (WRow_r = sum_c W1[r][c]). The host adds the 128*j offsets (msm_tail_finish).
 SPB_HD uint32_t msm_tail_partials(const MsmTail& t) { return 3 * t.nbr + 2 * t.nbc; }
 
-// (a): one group of buckets. `offsets` is the exclusive scan of the bucket counters (offsets[b+1] - offsets[b] entries in b).
+// (a): one group of buckets. offsets[b+1] - offsets[b] entries are in bucket b (step 3).
 SPB_HD void msm_group_thread(uint64_t tid, uint64_t ngroups, uint32_t m_log, const uint32_t* offsets, const G1Xyzz* buckets, G1Xyzz* s1, G1Xyzz* w1) {
   if (tid >= ngroups) return;
   const uint64_t b0 = tid << m_log;
@@ -316,64 +367,45 @@ inline G1Xyzz msm_tail_finish(const MsmGeom& g, const G1Xyzz* part) {
 
 #if defined(__CUDACC__) && defined(SPB_MSM_KERNELS)
 // ---- kernels --------------------------------------------------------------------------------------------
-// The number of sorted entries M is read from device memory (the last element of the offset scan), so the
-// whole MSM is enqueued without a host round trip between the sort and the accumulation.
-// Warp-aggregated versions of msm_count_thread / msm_scatter_thread: lanes whose digit lands in the same bucket
-// (witness columns are full of repeated small values) are found with match.any and served by ONE atomic, so a column
-// of equal scalars costs one atomic per warp and window instead of 32 serialised ones on the same address. The loop
-// is kept convergent (inactive lanes carry a flag instead of leaving) so the warp-level primitives are well defined.
-// Lanes of the warp holding the same key as the caller (inactive lanes pass kNoKey). MATCH.ANY costs tens of issue cycles per warp
-// and was what bound the histogram and sort kernels (ncu: top stall of msm_count / msm_bin_local_sort), while only columns
-// of repeated values need the grouping -- and those show equal keys in NEIGHBOURING lanes. So: one shuffle + vote decide; without
-// neighbouring duplicates every lane is its own group (any duplicates elsewhere in the warp just take their own atomics, which is
-// always correct -- the grouping is an optimisation).
-__device__ __forceinline__ unsigned msm_warp_peers(uint32_t key, uint32_t lane) {
-  const uint32_t next = __shfl_down_sync(0xffffffffu, key, 1);
-  const bool dup = lane < 31u && next == key && key != kNoKey;
-  if (__any_sync(0xffffffffu, dup)) return __match_any_sync(0xffffffffu, key);
-  return 1u << lane;
-}
-__global__ void msm_count_kernel(uint64_t n, const Fr* scalars, MsmGeom g, uint32_t* counts) {
+// The accumulation and every later kernel read the number of sorted entries M from device memory (the entry total the
+// digit kernel counts); the host reads it once per MSM, to give the radix sort its length.
+//
+// Step 1: one scalar per thread, 256 threads per block. The block's entries form one range reserved by ONE atomic on the
+// entry total (one atomic per warp would put eight times as many on that single address); inside it every warp writes its
+// entries window by window, so each store instruction of a warp covers consecutive entries. Digits are derived twice from the
+// canonical scalar (count, then write): shifts only, the Montgomery conversion is done once.
+static const unsigned kDigitsThreads = 256;
+__global__ void __launch_bounds__(kDigitsThreads) msm_digits_kernel(uint64_t n, const Fr* scalars, MsmGeom g, uint32_t* total, MsmEntry* ent) {
+  __shared__ uint32_t s_warp[kDigitsThreads / 32];
+  __shared__ uint32_t s_base;
   const uint64_t tid = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
-  const uint32_t lane = threadIdx.x & 31u;
+  const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
   bool live = tid < n;
   Fr s = live ? fp_from_mont(scalars[tid]) : fp_zero<FrParams>();
   live = live && !fp_is_zero(s);
+  uint32_t wsum = live ? msm_digit_count(s, g) : 0u;
+  for (int o = 16; o; o >>= 1) wsum += __shfl_xor_sync(0xffffffffu, wsum, o);
+  if (lane == 0) s_warp[warp] = wsum;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    uint32_t run = 0;
+    for (unsigned i = 0; i < kDigitsThreads / 32; i++) { const uint32_t v = s_warp[i]; s_warp[i] = run; run += v; }
+    s_base = run ? atomicAdd(total, run) : 0u;
+  }
+  __syncthreads();
+  uint32_t pos = s_base + s_warp[warp];
   DigitIter it; it.init(s, g.c);
   for (uint32_t w = 0; w < g.W; w++) {
-    int32_t d = it.next();
+    const int32_t d = it.next();
     const bool act = live && d != 0;
-    const uint32_t mag = d < 0 ? (uint32_t)(-d) : (uint32_t)d;
-    const uint32_t key = (g.precomp ? 0u : w * g.B) + mag - 1;
-    const unsigned peers = msm_warp_peers(act ? key : kNoKey, lane);
-    if (act && lane == (uint32_t)(__ffs(peers) - 1)) atomicAdd(&counts[key], (uint32_t)__popc(peers));
+    const unsigned m = __ballot_sync(0xffffffffu, act);
+    if (act) ent[pos + (uint32_t)__popc(m & ((1u << lane) - 1u))] = msm_make_entry(tid, w, d, g);
+    pos += (uint32_t)__popc(m);
   }
 }
-__global__ void msm_scatter_kernel(uint64_t n, const Fr* scalars, MsmGeom g, uint32_t* cursor, MsmEntry* ent) {
-  const uint64_t tid = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
-  const uint32_t lane = threadIdx.x & 31u;
-  bool live = tid < n;
-  Fr s = live ? fp_from_mont(scalars[tid]) : fp_zero<FrParams>();
-  live = live && !fp_is_zero(s);
-  DigitIter it; it.init(s, g.c);
-  for (uint32_t w = 0; w < g.W; w++) {
-    int32_t d = it.next();
-    const bool act = live && d != 0;
-    const uint32_t mag = d < 0 ? (uint32_t)(-d) : (uint32_t)d;
-    const uint32_t key = (g.precomp ? 0u : w * g.B) + mag - 1;
-    // whole-warp match and shuffle (inactive lanes carry a key no bucket has): a shuffle under per-group masks would be executed
-    // once per group -- 32 times for 32 distinct keys
-    const unsigned peers = msm_warp_peers(act ? key : kNoKey, lane);
-    const uint32_t leader = (uint32_t)(__ffs(peers) - 1);
-    uint32_t base = 0;
-    if (act && lane == leader) base = atomicAdd(&cursor[key], (uint32_t)__popc(peers));
-    base = __shfl_sync(0xffffffffu, base, leader);
-    if (act) {
-      const uint32_t pos = base + (uint32_t)__popc(peers & ((1u << lane) - 1u));
-      MsmEntry e; e.key = key; e.val = ((uint32_t)tid + (g.precomp ? w * g.tab_stride : 0u)) | (d < 0 ? 0x80000000u : 0u);
-      ent[pos] = e;
-    }
-  }
+// Step 3: one thread per bucket k in [0, nb].
+__global__ void __launch_bounds__(256) msm_offsets_kernel(const uint32_t* total, uint64_t nb, const MsmEntry* sorted, uint32_t* offsets) {
+  msm_offsets_thread(blockIdx.x * (uint64_t)blockDim.x + threadIdx.x, nb, *total, sorted, offsets);
 }
 #ifndef SPB_ACC_MINBLOCKS
 #define SPB_ACC_MINBLOCKS 1

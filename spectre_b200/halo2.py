@@ -163,7 +163,7 @@ class Backend:
     def last_msm_stage_ms(self):
         out = (ctypes.c_float * 7)()
         self.lib.spb_last_msm_stage_ms(self.ctx, out)
-        return dict(zip(("count", "scan", "scatter", "accumulate", "stitch", "groups", "rowcol_weighted"), [float(v) for v in out]))
+        return dict(zip(("digits", "sort", "offsets", "accumulate", "stitch", "groups", "rowcol_weighted"), [float(v) for v in out]))
 
     def msm_geometry(self, n, tables=False):
         c = ctypes.c_uint32(); w = ctypes.c_uint32()
