@@ -110,6 +110,12 @@ void spb_srs_free(spb_ctx* ctx, spb_srs* srs);
  * (g_to_lagrange: the inverse DFT over the group, on the device; no knowledge of the secret needed). The reference keeps
  * a degree -> params map for exactly this (prover/src/prover.rs:34). Returns a NEW handle without window tables. */
 int spb_srs_downsize(spb_ctx* ctx, const spb_srs* srs, uint32_t k, spb_srs** out);
+/* A powers-of-tau update of a 2^k SRS by the secret t (Montgomery limbs, 0 < t < r): a NEW handle (no window tables) with
+ * g'[j] = t^j g[j], g_lagrange' = g_to_lagrange(g'), g2' = g2, s_g2' = t s_g2 -- ParamsKZG::setup run by several parties, each
+ * of which applies its own t; nobody learns the final secret unless every party's t is known. The input handle is not
+ * modified. SPB_ERR_ARG: a NULL argument, t = 0 or t >= r; SPB_ERR_STATE: a spb_bases_upload handle, a handle with window
+ * tables, or a handle whose G2 trailer is zero (spb_srs_set_g2 first). spb_last_device_ms: the scaling and g_to_lagrange. */
+int spb_srs_contribute(spb_ctx* ctx, const spb_srs* srs, const spb_fr* t, spb_srs** out);
 /* ParamsKZG::read_custom / ::write: k (u32 LE) | g[2^k] | g_lagrange[2^k] | g2 | s_g2 with every coordinate as its
  * in-memory Montgomery limbs -- the `params/kzg_bn254_{k}.srs` file halo2-base's gen_srs caches (reference:
  * prover/src/cli.rs:48, .gitignore:36). The read streams the points straight into device memory.

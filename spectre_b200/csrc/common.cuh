@@ -185,6 +185,9 @@ int stream_device_to_file(spb_ctx* ctx, DeviceState& d, FILE* f, const void* d_s
 // ---- msm.cu ----
 void msm_release_ctx(spb_ctx* ctx);
 
+// ---- pairing.cu: out = t in for a G2 point of a params trailer (128 bytes, Montgomery limbs; t Montgomery), on the host ----
+void g2_trailer_mul(unsigned char out[128], const unsigned char in[128], const Fr& t);
+
 // ---- ntt.cu ----
 struct NttOpts {
   uint64_t n_in = 0, n_out = 0;  // 0 = n

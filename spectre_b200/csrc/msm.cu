@@ -399,7 +399,10 @@ fail:
 // g_to_lagrange(g) = the inverse DFT over the group (log2 n stages of n/2 butterflies, each one point addition, one
 // subtraction and one 254-bit scalar multiple by a power of omega^-1; then 1/n and affine normalisation). Works for any SRS
 // (no knowledge of the secret). Returns a NEW handle (no window tables); the caller frees the old one when it is done with it.
-static int srs_downsize_locked(spb_ctx* ctx, const spb_srs* srs, uint32_t k, spb_srs** made) {
+//
+// g_to_lagrange of the first n = 2^k points of src's g (complete before the call), on the context's first device: the points
+// gathered into slot "ds_g", the result in slot "ds_lag". Enqueued on that device's stream, not waited for.
+static int srs_g_to_lagrange(spb_ctx* ctx, const spb_srs* src, uint32_t k, const char* who, G1Affine** g_out, G1Affine** lag_out) {
   const uint64_t n = 1ull << k;
   DeviceState& d = ctx->dev[0];
   SPB_CUDA(ctx, cudaSetDevice(d.device));
@@ -408,9 +411,9 @@ static int srs_downsize_locked(spb_ctx* ctx, const spb_srs* srs, uint32_t k, spb
   G1Affine* lag = (G1Affine*)slot(ctx, d, "ds_lag", n * sizeof(G1Affine));
   Fr* tw = (Fr*)slot(ctx, d, "ds_tw", (n / 2 ? n / 2 : 1) * sizeof(Fr));
   if (!g0 || !pts || !lag || !tw) return SPB_ERR_OOM;
-  for (auto& sh : srs->shards) {
+  for (auto& sh : src->shards) {
     if (sh.start >= n || !sh.count) continue;
-    if (!sh.g) return set_error(ctx, SPB_ERR_STATE, "spb_srs_downsize: basis g not resident");
+    if (!sh.g) return set_error(ctx, SPB_ERR_STATE, "%s: basis g not resident", who);
     const size_t cnt = (n - sh.start) < sh.count ? (n - sh.start) : sh.count;
     SPB_CUDA(ctx, cudaMemcpyPeerAsync(g0 + sh.start, d.device, sh.g, ctx->dev[sh.dev_index].device, cnt * sizeof(G1Affine), d.stream));
   }
@@ -422,25 +425,73 @@ static int srs_downsize_locked(spb_ctx* ctx, const spb_srs* srs, uint32_t k, spb
     for (uint64_t half = n / 2; half >= 1; half >>= 1) SPB_TRY(launch(ctx, d.stream, nblk(n / 2, tb), tb, 0, ec_ntt_stage_kernel, n, half, tw, pts));
   }
   SPB_TRY(launch(ctx, d.stream, nblk(n, tb), tb, 0, ec_ntt_finish_kernel, n, k, n_inv, pts, lag));
-  spb_srs* s = srs_alloc(ctx, k);
-  *made = s;
-  memcpy(s->g2, srs->g2, 128); memcpy(s->s_g2, srs->s_g2, 128);
+  *g_out = g0; *lag_out = lag;
+  return 0;
+}
+
+// Give every shard of s its g_lagrange (and its g, when g is not null) from the first device's buffers, and wait for the copies.
+static int srs_fill_shards(spb_ctx* ctx, spb_srs* s, const G1Affine* g, const G1Affine* lag, const char* who) {
+  DeviceState& d = ctx->dev[0];
   cudaError_t e = cudaSuccess;
   for (auto& sh : s->shards) {
     if (!sh.count) continue;
     DeviceState& dd = ctx->dev[sh.dev_index];
     e = cudaSetDevice(dd.device);
-    if (e == cudaSuccess) e = cudaMalloc(&sh.g, sh.count * sizeof(G1Affine));
+    if (e == cudaSuccess && g) e = cudaMalloc(&sh.g, sh.count * sizeof(G1Affine));
     if (e == cudaSuccess) e = cudaMalloc(&sh.g_lagrange, sh.count * sizeof(G1Affine));
     if (e != cudaSuccess) break;
     cudaSetDevice(d.device);
-    e = cudaMemcpyPeerAsync(sh.g, dd.device, g0 + sh.start, d.device, sh.count * sizeof(G1Affine), d.stream);
+    if (g) e = cudaMemcpyPeerAsync(sh.g, dd.device, g + sh.start, d.device, sh.count * sizeof(G1Affine), d.stream);
     if (e == cudaSuccess) e = cudaMemcpyPeerAsync(sh.g_lagrange, dd.device, lag + sh.start, d.device, sh.count * sizeof(G1Affine), d.stream);
     if (e != cudaSuccess) break;
   }
   cudaSetDevice(d.device);
   if (e == cudaSuccess) e = cudaStreamSynchronize(d.stream);
-  if (e != cudaSuccess) return set_error(ctx, SPB_ERR_CUDA, "spb_srs_downsize: %s", cudaGetErrorString(e));
+  if (e != cudaSuccess) return set_error(ctx, SPB_ERR_CUDA, "%s: %s", who, cudaGetErrorString(e));
+  return 0;
+}
+
+static int srs_downsize_locked(spb_ctx* ctx, const spb_srs* srs, uint32_t k, spb_srs** made) {
+  G1Affine *g0, *lag;
+  SPB_TRY(srs_g_to_lagrange(ctx, srs, k, "spb_srs_downsize", &g0, &lag));
+  spb_srs* s = srs_alloc(ctx, k);
+  *made = s;
+  memcpy(s->g2, srs->g2, 128); memcpy(s->s_g2, srs->s_g2, 128);
+  return srs_fill_shards(ctx, s, g0, lag, "spb_srs_downsize");
+}
+
+// ParamsKZG::setup run by several parties: one powers-of-tau update by the secret t. Each shard scales its own points on its own
+// device (srs_scale_kernel, global index start + j), g_lagrange is g_to_lagrange of the new g at the handle's own k (the path
+// of downsize), and s_g2 = t s_g2 on the host. last_kernel_ms: first scaling launch to the end of g_to_lagrange, on the first
+// device's clock.
+static int srs_contribute_locked(spb_ctx* ctx, const spb_srs* srs, const Fr& t, spb_srs** made) {
+  spb_srs* s = srs_alloc(ctx, srs->k);
+  *made = s;
+  DeviceState& d0 = ctx->dev[0];
+  SPB_CUDA(ctx, cudaSetDevice(d0.device));
+  SPB_CUDA(ctx, cudaEventRecord(d0.ev0, d0.stream));
+  for (size_t i = 0; i < s->shards.size(); i++) {
+    const SrsShard& from = srs->shards[i];
+    SrsShard& to = s->shards[i];
+    if (!to.count) continue;
+    if (!from.g) return set_error(ctx, SPB_ERR_STATE, "spb_srs_contribute: basis g not resident");
+    DeviceState& d = ctx->dev[to.dev_index];
+    SPB_CUDA(ctx, cudaSetDevice(d.device));
+    SPB_CUDA(ctx, cudaMalloc(&to.g, to.count * sizeof(G1Affine)));
+    SPB_TRY(launch(ctx, d.stream, nblk(to.count, 128), 128, 0, srs_scale_kernel, (uint64_t)to.start, (uint64_t)to.count, t, (const G1Affine*)from.g, to.g));
+  }
+  for (auto& sh : s->shards) {
+    if (!sh.count) continue;
+    SPB_CUDA(ctx, cudaSetDevice(ctx->dev[sh.dev_index].device));
+    SPB_CUDA(ctx, cudaStreamSynchronize(ctx->dev[sh.dev_index].stream));
+  }
+  G1Affine *g0, *lag;
+  SPB_TRY(srs_g_to_lagrange(ctx, s, s->k, "spb_srs_contribute", &g0, &lag));
+  SPB_CUDA(ctx, cudaEventRecord(d0.ev1, d0.stream));
+  SPB_TRY(srs_fill_shards(ctx, s, nullptr, lag, "spb_srs_contribute"));
+  SPB_CUDA(ctx, cudaEventElapsedTime(&ctx->last_kernel_ms, d0.ev0, d0.ev1));
+  memcpy(s->g2, srs->g2, 128);
+  g2_trailer_mul(s->s_g2, srs->s_g2, t);
   return 0;
 }
 int spb_srs_downsize(spb_ctx* ctx, const spb_srs* srs, uint32_t k, spb_srs** out) {
@@ -450,6 +501,24 @@ int spb_srs_downsize(spb_ctx* ctx, const spb_srs* srs, uint32_t k, spb_srs** out
   spb_srs* made = nullptr;
   int rc;
   { std::lock_guard<std::mutex> lk(ctx->mu); rc = srs_downsize_locked(ctx, srs, k, &made); }
+  if (rc != 0) { if (made) spb_srs_free(ctx, made); return rc; }
+  *out = made;
+  return 0;
+}
+
+int spb_srs_contribute(spb_ctx* ctx, const spb_srs* srs, const spb_fr* t, spb_srs** out) {
+  if (!ctx || !srs || !t || !out) return SPB_ERR_ARG;
+  const Fr tm = fr_load(t);
+  if (fp_is_zero(tm)) return set_error(ctx, SPB_ERR_ARG, "spb_srs_contribute: t = 0 would erase every point after g[0]");
+  if (!fp_is_canonical(tm)) return set_error(ctx, SPB_ERR_ARG, "spb_srs_contribute: t is not less than r");
+  if (srs->n != ((size_t)1 << srs->k)) return set_error(ctx, SPB_ERR_STATE, "spb_srs_contribute: the handle holds %zu plain bases (spb_bases_upload), not a 2^k SRS", srs->n);
+  if (srs->table_c) return set_error(ctx, SPB_ERR_STATE, "spb_srs_contribute: call before spb_srs_precompute (the table rows replaced the plain basis layout)");
+  static const unsigned char zero[128] = {0};
+  if (!memcmp(srs->g2, zero, 128) || !memcmp(srs->s_g2, zero, 128))
+    return set_error(ctx, SPB_ERR_STATE, "spb_srs_contribute: the handle's G2 trailer is zero (give it with spb_srs_set_g2 first)");
+  spb_srs* made = nullptr;
+  int rc;
+  { std::lock_guard<std::mutex> lk(ctx->mu); rc = srs_contribute_locked(ctx, srs, tm, &made); }
   if (rc != 0) { if (made) spb_srs_free(ctx, made); return rc; }
   *out = made;
   return 0;

@@ -630,7 +630,28 @@ SPB_HD void ec_ntt_finish_thread(uint64_t tid, uint64_t n, uint32_t k, const Fr&
   for (uint32_t b = 0; b < k; b++) r |= ((tid >> b) & 1ull) << (k - 1 - b);
   out[tid] = xyzz_to_affine(xyzz_mul_scalar(p[r], fp_from_mont(scale)));
 }
+
+// ---- spb_srs_contribute: a powers-of-tau update g'[j] = t^j g[j] -----------------------------------------------------------
+// point `tid` of a shard whose first point has global index `start`: out = t^(start + tid) in, affine. xyzz_mul_scalar's
+// MSB-first double-and-add with mixed additions (the base is affine); the power is computed per thread (at most 2 log2 n
+// products, against about 3800 for the multiple). The identity stays the identity.
+SPB_HD void srs_scale_thread(uint64_t tid, uint64_t start, uint64_t n, const Fr& t, const G1Affine* in, G1Affine* out) {
+  if (tid >= n) return;
+  const Fr k = fp_from_mont(fp_pow_u64(t, start + tid));
+  const G1Affine p = in[tid];
+  int top = 255;
+  while (top >= 0 && !((k.l[top >> 5] >> (top & 31)) & 1)) top--;
+  G1Xyzz r = xyzz_identity();
+  for (int i = top; i >= 0; i--) {
+    r = xyzz_dbl(r);
+    if ((k.l[i >> 5] >> (i & 31)) & 1) xyzz_add_mixed(r, p);
+  }
+  out[tid] = xyzz_to_affine(r);
+}
 #if defined(__CUDACC__) && defined(SPB_MSM_KERNELS)
+__global__ void __launch_bounds__(128) srs_scale_kernel(uint64_t start, uint64_t n, Fr t, const G1Affine* in, G1Affine* out) {
+  srs_scale_thread(blockIdx.x * (uint64_t)blockDim.x + threadIdx.x, start, n, t, in, out);
+}
 __global__ void __launch_bounds__(128) ec_lift_kernel(uint64_t n, const G1Affine* in, G1Xyzz* out) {
   uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
   if (i < n) out[i] = xyzz_from_affine(in[i]);

@@ -45,6 +45,13 @@ __global__ void __launch_bounds__(32) pairing_final_kernel(const Fq12* f, uint64
   if (ok) ok[j] = fq12_is_one(acc) ? 1 : 0;
 }
 
+void g2_trailer_mul(unsigned char out[128], const unsigned char in[128], const Fr& t) {
+  G2Affine q;
+  memcpy(&q, in, sizeof q);
+  q = g2_mul_scalar(q, fp_from_mont(t));
+  memcpy(out, &q, sizeof q);
+}
+
 static const unsigned kPairingThreads = 32;  // small blocks: a few hundred pairs already spread over every SM
 
 static const char* pairing_point_reason(int verdict) {

@@ -279,6 +279,23 @@ SPB_HD_NOINLINE bool g2_in_subgroup(const G2Affine& q) {
   return fq2_is_zero(t.z);
 }
 
+// k Q for a canonical (non-Montgomery) scalar k, as an affine point (identity (0, 0)): MSB-first double-and-add over the steps
+// of g2_in_subgroup, then one Fq2 inversion. The G2 trailer of a powers-of-tau update (spb_srs_contribute), run on the host.
+SPB_HD_NOINLINE G2Affine g2_mul_scalar(const G2Affine& q, const Fr& k) {
+  G2Proj t; t.x = fq2_zero(); t.y = fq2_one(); t.z = fq2_zero();
+  if (!g2_affine_is_identity(q))
+    for (int i = 255; i >= 0; i--) {
+      if (!fq2_is_zero(t.z)) g2_dbl_step(t, nullptr, nullptr, nullptr, fp_zero<FqParams>(), fp_zero<FqParams>());
+      if ((k.l[i >> 5] >> (i & 31)) & 1) g2_add_complete(t, q);
+    }
+  G2Affine r; r.x = fq2_zero(); r.y = fq2_zero();
+  if (fq2_is_zero(t.z)) return r;
+  const Fq2 zi = fq2_inv(t.z);
+  r.x = fq2_mul(t.x, zi);
+  r.y = fq2_mul(t.y, zi);
+  return r;
+}
+
 // The input check of a pairing's G2 point: g2_affine_check (canonical, on the twist), then membership in the order-r subgroup.
 SPB_HD int g2_pairing_check(const G2Affine& q) {
   const int v = g2_affine_check(q);

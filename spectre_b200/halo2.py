@@ -670,6 +670,16 @@ class ParamsKZG:
         self.be.check(self.be.lib.spb_srs_downsize(self.be.ctx, self.h, ctypes.c_uint32(k), ctypes.byref(h)), "spb_srs_downsize")
         return ParamsKZG(self.be, k, h)
 
+    def contribute(self, t):
+        """One powers-of-tau update by the secret t (Montgomery limbs, 0 < t < r; spb_srs_contribute): a new handle with g[j]
+        t^j g[j], g_lagrange = g_to_lagrange of that g, and the trailer's s_g2 times t, all computed on the device(s). The handle
+        needs its G2 trailer (set_g2) and no window tables; it stays valid and unchanged. plonk.contribute_params wraps this with
+        the public record of the update."""
+        t = _fr_array(t, 1)
+        h = ctypes.c_void_p()
+        self.be.check(self.be.lib.spb_srs_contribute(self.be.ctx, self.h, _p(t), ctypes.byref(h)), "spb_srs_contribute")
+        return ParamsKZG(self.be, self.k, h)
+
     def write(self, path):
         self.be.check(self.be.lib.spb_srs_write_file(self.be.ctx, self.h, path.encode()), "spb_srs_write_file")
 

@@ -1312,6 +1312,122 @@ def check_params(E, be, vp=None, seed=None, timings=None):
     return failures
 
 
+# ---- multi-party params: a powers-of-tau update chain ---------------------------------------------------------------
+# Each party i draws t_i, maps g[j] -> t_i^j g[j] and [s]_2 -> t_i [s]_2 (ParamsKZG.contribute) and publishes a ParamsUpdate.
+# If any one party erased its t_i, nobody knows the final secret s_0 t_1 ... t_m, whoever made the starting params.
+PARAMS_UPDATE_DOMAIN = b"spectre-b200 params update v1"
+PARAMS_UPDATE_BYTES = 128 + 64 + 64 + 32
+
+
+class ParamsUpdate(namedtuple("ParamsUpdate", "s_g2 t_g1 r_g1 z")):
+    """The public record of one powers-of-tau update: s_g2 = [s]_2 after the update (uint64[16], the params trailer's layout),
+    t_g1 = T = t G1 and r_g1 = R = rho G1 (uint64[8] each, G1 affine limbs) and z = rho + c t mod r (an int), a Schnorr proof
+    that the party knew t, with c = params_update_challenge(the [s]_2 before, this record).
+
+    to_bytes / from_bytes: s_g2 (128 B) | T (64 B) | R (64 B) | z (32 B). Every coordinate is its Montgomery limbs as the params
+    file's trailer stores them, and z is its Fr Montgomery limbs, all little-endian."""
+
+    def to_bytes(self):
+        return b"".join(np.ascontiguousarray(a, dtype="<u8").tobytes() for a in (self.s_g2, self.t_g1, self.r_g1, fr_mont(self.z)))
+
+    @classmethod
+    def from_bytes(cls, data):
+        """The inverse of to_bytes. ValueError for a wrong length, a coordinate or z not canonical, or a G1 point off the curve
+        (the G2 point's curve and subgroup are checked where the pairing takes it)."""
+        data = bytes(data)
+        if len(data) != PARAMS_UPDATE_BYTES:
+            raise ValueError("ParamsUpdate.from_bytes: %d bytes, the record is %d" % (len(data), PARAMS_UPDATE_BYTES))
+        if any(int.from_bytes(data[i:i + 32], "little") >= P_MOD for i in range(0, 128, 32)):
+            raise ValueError("ParamsUpdate.from_bytes: s_g2: a coordinate is not less than the field modulus")
+        for name, raw in (("T", data[128:192]), ("R", data[192:256])):
+            why = _point_check(raw)
+            if why:
+                raise ValueError("ParamsUpdate.from_bytes: %s: %s" % (name, why))
+        if int.from_bytes(data[256:], "little") >= R_MOD:
+            raise ValueError("ParamsUpdate.from_bytes: z is not less than r")
+        return cls(_limbs(data[:128]), _limbs(data[128:192]), _limbs(data[192:256]), fr_int(_limbs(data[256:])))
+
+
+def params_update_challenge(s_g2_before, update):
+    """c = keccak256(b"spectre-b200 params update v1" || s_g2 before || s_g2 after || T || R), read big-endian, mod r, each point
+    in the bytes of ParamsUpdate.to_bytes. This is this project's own encoding, not an external standard: a record is checked
+    only by this code. Binding the [s]_2 before makes a record valid at its own place in the chain only."""
+    data = PARAMS_UPDATE_DOMAIN + b"".join(np.ascontiguousarray(a, dtype="<u8").tobytes() for a in (s_g2_before, update.s_g2, update.t_g1, update.r_g1))
+    return int.from_bytes(keccak256(data), "big") % R_MOD
+
+
+def prove_params_update(be, s_g2_before, s_g2_after, t, rho):
+    """The ParamsUpdate of the update by t from s_g2_before to s_g2_after, with the Schnorr nonce rho (ints in [1, r)). be:
+    anything with best_multiexp(coeffs, bases) in halo2.Backend's layouts."""
+    t_g1, r_g1 = (_g1_limbs(_multiexp(be, [v], [(1, 2)])) for v in (t, rho))
+    update = ParamsUpdate(np.asarray(s_g2_after, dtype=np.uint64).reshape(16).copy(), t_g1, r_g1, 0)
+    return update._replace(z=(rho + params_update_challenge(s_g2_before, update) * t) % R_MOD)
+
+
+def _random_fr():
+    """Fr::random's rule: 64 bytes of os.urandom read little-endian, reduced mod r (from_u512)"""
+    return int.from_bytes(os.urandom(64), "little") % R_MOD
+
+
+def contribute_params(be, params, secret=None, nonce=None):
+    """One party's powers-of-tau update of params (a halo2.ParamsKZG with its G2 trailer and no window tables): returns
+    (new params, ParamsUpdate). secret = t and nonce = rho, ints in [1, r), are drawn as Fr::random draws them when None. The
+    input params stay valid and unchanged.
+
+    The party must erase t (and rho) afterwards: anyone who learns every party's t can forge proofs. Python cannot scrub
+    memory (ints are immutable and may be copied), so a caller who needs erasure runs the contribution in a process that exits
+    once it has written the new params file and the record."""
+    t = _random_fr() if secret is None else secret
+    rho = _random_fr() if nonce is None else nonce
+    if not 0 < t < R_MOD or not 0 < rho < R_MOD:
+        raise ValueError("contribute_params: the secret and the nonce must lie in [1, r)")
+    s_before = params.get_g2()[1]
+    new = params.contribute(fr_mont(t))
+    return new, prove_params_update(be, s_before, new.get_g2()[1], t, rho)
+
+
+class UpdateFailure(namedtuple("UpdateFailure", "kind index detail")):
+    """One failing record of a params update chain (check_params_updates), index = its place in the chain. At most one per record,
+    the first of:
+      "degenerate": T or the record's s_g2 is the identity;
+      "ratio": e(T, s_before) != e(G1, s_g2): the record's [s]_2 is not t times the one before it (a record out of place, a T
+        for another t, or an s_g2 that does not follow);
+      "knowledge": z G1 != R + c T, so the record does not prove that its party knew t.
+    detail: a human-readable reason."""
+
+
+def check_params_updates(E, be, start_vp, updates, seed=None):
+    """Check a powers-of-tau update chain and the params it ends in: a list of UpdateFailure in chain order, then the ParamsFailure
+    list of check_params against [s]_2 of the last record; [] for a sound chain. E: an engine bound to the final params; be:
+    anything with best_multiexp and pairing_check_batch in halo2.Backend's layouts; start_vp: the ParamsVerifierKZG of the params
+    the chain starts from (s_0 = start_vp.s_g2); updates: the ParamsUpdate records in order; seed: check_params' seed.
+
+    Per record, one 3-term best_multiexp decides knowledge (z G1 - c T - R = O). Every ratio check e(T_i, s_{i-1}) e(-G1, s_i) = 1
+    goes into one pairing_check_batch call of len(updates) checks of two pairs. Then check_params(E, be, ParamsVerifierKZG(G1,
+    start_vp.g2, s_m)) shows that the final params are the powers of that s_m."""
+    generator, neg_generator = _g1_limbs((1, 2)), _g1_limbs((1, P_MOD - 2))
+    prev = np.asarray(start_vp.s_g2, dtype=np.uint64).reshape(16)
+    ps, qs, found = [], [], []
+    for i, u in enumerate(updates):
+        s_after = np.asarray(u.s_g2, dtype=np.uint64).reshape(16)
+        if not np.asarray(u.t_g1).any() or not s_after.any():
+            found.append(UpdateFailure("degenerate", i, "T is the identity" if not np.asarray(u.t_g1).any() else "s_g2 is the identity"))
+        else:
+            c = params_update_challenge(prev, u)
+            rest = halo2.jacobian_to_affine_ints(be.best_multiexp(fr_mont_rows([u.z, R_MOD - c, R_MOD - 1]), np.stack([generator, u.t_g1, u.r_g1])))
+            found.append(None if rest == (0, 0) else UpdateFailure("knowledge", i, "z G1 is not R + c T"))
+        ps += [u.t_g1, neg_generator]
+        qs += [prev, s_after]
+        prev = s_after
+    if updates:
+        ok = be.pairing_check_batch(np.stack(ps), np.stack(qs), 2)
+        for i, holds in enumerate(ok):
+            if not holds and (found[i] is None or found[i].kind != "degenerate"):
+                found[i] = UpdateFailure("ratio", i, "s_g2 of record %d is not t s_g2 of the one before it" % i)
+    failures = [f for f in found if f is not None]
+    return failures + check_params(E, be, halo2.ParamsVerifierKZG(generator, start_vp.g2, prev), seed=seed)
+
+
 # ---- verifier -----------------------------------------------------------------------------------------------------
 # [UPSTREAM] halo2_proofs/src/plonk/verifier.rs verify_proof with VerifierSHPLONK and SingleStrategy
 # (poly/kzg/multiopen/shplonk/verifier.rs, poly/kzg/strategy.rs): what snark_verifier_sdk::gen_proof runs on every proof it
